@@ -1,10 +1,17 @@
 #!/usr/bin/env python
-"""bench.py — RNN-T loss+grad throughput on B200 (BASELINE.json metric), one JSON line.
+"""bench.py — RNN-T loss+grad throughput on H100 (BASELINE.json metric), one JSON line.
 
     python bench.py --gpus 1 --steps 20 --warmup 3                      # our arm, 1 GPU
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W       # our arm, N GPUs (weak scaling)
     python bench.py --impl reference --gpus 1 --steps K --warmup W      # reference CPU path on host cores
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR    # + the last timed step's outputs
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed: DIR/costs.npy
+(float32 [N] per-utterance losses), DIR/loss.npy (float32 [1], their sum) and DIR/grads_sample.npy
+(float32, the logits-gradient at DUMP_SAMPLES flat positions drawn with numpy seed DUMP_SEED, in
+increasing order).  The synthetic inputs are seeded, so two builds run with the same arguments can be
+compared output for output.
 
 A step = one pass of the hot path (log-softmax statistics -> alpha/beta lattice -> dense gradient)
 over one batch of synthetic logits; workload = BASELINE config "N=128, T=150, L=20, A=5000 fp32"
@@ -16,13 +23,14 @@ value         device-resident: inputs already in HBM, compute_rnnt_loss_async + 
 e2e           through the reference-facing C-ABI call compute_rnnt_loss() (host-synchronous, costs to
               the host) with the step's logits coming from pinned host memory inside the timed region.
 roofline      the dominant kernel (grad_row_kernel, 8 B/element algorithmic) timed with CUDA events on the
-              library's own stream during the timed steps, against MEASURED_PEAKS.json.
+              library's own stream during the timed steps, against MEASURED_PEAKS.json (else the H100 SXM
+              data-sheet 3.35 TB/s).
 parity_check  after the timed region, on EVERY rank: two utterances of the rank's shard (one full-length,
               one ragged) against the fp64 CPU oracle, and all_reduce(loss) == sum(all_gather(local sums)).
 c5_strong     BASELINE config 5 as written: 1024 utterances (T=200, L=40, A=5000) split over the G ranks,
               each rank streaming 1024/G/128 micro-batches of 128 utterances through ONE fixed set of
               activation / gradient / workspace buffers per step, one all-reduce per step (strong scaling).
-reference_gpu the reference's own CUDA kernels (oracle/_ref/libwarprnnt_ref_gpu.so, built for sm_100 from
+reference_gpu the reference's own CUDA kernels (oracle/_ref/libwarprnnt_ref_gpu.so, built for sm_90 from
               the unmodified reference sources) on the same inputs, tests/test_time.cu's 10-call protocol.
 other_workloads  BASELINE configs 2, 4, the config-5 shard, bf16 logits at config 3 and the additive-joint
               training step, each with ms, utt/s and its recomputed roofline fraction (N=1 only).
@@ -48,8 +56,11 @@ WORKLOADS = {   # name: (N per GPU, T, L, V)   BASELINE.json configs
     "c5": (128, 200, 40, 5000),     # config 5's micro-batch: 1024 utterances in slabs of 128
 }
 C5_GLOBAL_BATCH = 1024
+DUMP_SAMPLES = 1 << 22     # 16 MB of float32 gradient values
+DUMP_SEED = 20261015
 METRIC = "RNN-T loss+grad utterances/s at T=150,L=20,A=5000"
 UNIT = "utterances/s"
+HBM_DATASHEET_GBS = 3350.0   # H100 SXM, HBM3
 
 
 def gen_labels(V, L, N):
@@ -67,7 +78,7 @@ def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": HBM_DATASHEET_GBS}, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -120,8 +131,8 @@ class ClockSampler(threading.Thread):
 def bind_to_gpu_numa_node(index):
     """Pin this process to the CPUs local to GPU `index` (NVML's CPU affinity = the GPU's NUMA node)
     BEFORE any pinned host memory is allocated, so the step's 8 GB staging buffer is first-touched on
-    the memory controller next to the GPU's PCIe root.  Round 1: with 8 ranks and no placement the
-    pinned-host -> device streams of GPUs 4-7 crossed the socket link and e2e scaled 0.77."""
+    the memory controller next to the GPU's PCIe root: without placement the pinned-host -> device
+    streams of GPUs on the far socket cross the socket link."""
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -251,7 +262,7 @@ def workload_config(name, world):
     return {"workload": "%s: N=%d per GPU, T=%d, L=%d (U=%d), A=%d, fp32 logits ~U[0,1), full lengths, blank 0"
                         % (name, N, T, L, L + 1, V),
             "global_batch": N * world, "parallelism": "batch-sharded x%d" % world,
-            "l2": ("no flush: per-step inputs (%.2f GB logits) exceed the 126 MB L2" % (N * T * (L + 1) * V * 4 / 1e9))
+            "l2": ("no flush: per-step inputs (%.2f GB logits) exceed the 50 MB L2" % (N * T * (L + 1) * V * 4 / 1e9))
                   if needs_no_flush(name) else "L2 flushed (256 MB write) before every timed step; steps timed individually"}
 
 
@@ -370,7 +381,7 @@ def parity_leg(torch, dist, wr, sh, world, rank, dev):
 
 def c5_strong_leg(torch, dist, wr, world, rank, dev, steps):
     """BASELINE config 5 as written (N=1024, T=200, L=40, A=5000 fp32 over G GPUs): 168 GB of logits and
-    as much gradient do not fit one B200, so every rank streams its 1024/G utterances as micro-batches
+    as much gradient do not fit one H100 (80 GB), so every rank streams its 1024/G utterances as micro-batches
     of 128 through ONE fixed activation / gradient / workspace set per step (the producer - here a
     device-side refresh of the logits is NOT simulated: the synthetic slab is reused, the kernels read
     and write the full 21 GB + 21 GB per micro-batch from HBM), costs accumulate on the device and one
@@ -413,7 +424,7 @@ def c5_strong_leg(torch, dist, wr, world, rank, dev, steps):
            "micro_batch": 128, "ms_per_step": ms, "value": C5_GLOBAL_BATCH / (ms * 1e-3), "unit": UNIT,
            "steps": steps, "per_gpu_algorithmic_GBps": per_gpu_bytes / (ms * 1e-3) / 1e9,
            "loss_sum": loss, "buffers": "one fixed 21 GB logits + 21 GB gradient + workspace set per rank",
-           "note": "strong-scaling efficiency = ms_per_step(G=1) / (G * ms_per_step(G)), from the driver's per-G runs"}
+           "note": "strong-scaling efficiency = ms_per_step(G=1) / (G * ms_per_step(G)), from runs at each G"}
     del sh
     torch.cuda.empty_cache()
     return out
@@ -421,7 +432,7 @@ def c5_strong_leg(torch, dist, wr, world, rank, dev, steps):
 
 def reference_gpu_leg(torch, wr, dev, names):
     """tests/test_time.cu's protocol (3 untimed + 10 timed calls, wall clock around the host-synchronous
-    compute_rnnt_loss) on the reference's own CUDA kernels compiled for sm_100, and on this library, on the
+    compute_rnnt_loss) on the reference's own CUDA kernels compiled for sm_90, and on this library, on the
     same device-resident inputs."""
     import ctypes as C
     from oracle import pyoracle
@@ -432,7 +443,7 @@ def reference_gpu_leg(torch, wr, dev, names):
     ref.compute_rnnt_loss.restype = C.c_int
     ref.compute_rnnt_loss.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p, wr.rnntOptions]
     ref.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
-    out = {"lib": "oracle/_ref/libwarprnnt_ref_gpu.so (unmodified reference CUDA kernels, -arch sm_100)",
+    out = {"lib": "oracle/_ref/libwarprnnt_ref_gpu.so (unmodified reference CUDA kernels, -arch sm_90)",
            "protocol": "tests/test_time.cu:89-128: 3 warm-up + 10 timed host-synchronous calls, wall clock"}
     for name in names:
         sh = Shard(torch, wr, dev, name, 99)
@@ -491,12 +502,12 @@ def other_workloads_leg(torch, wr, dev, peaks):
             out[key] = {"workload": "N=%d T=%d L=%d A=%d %s" % (sh.N, sh.T, sh.L, sh.V, "bf16 logits+grads, fp32 math" if dtype else "fp32"),
                         "ms_per_step": ms, "value": sh.N / (ms * 1e-3), "unit": UNIT,
                         "algorithmic_GBps": bytes_ / (ms * 1e-3) / 1e9, "frac_of_measured_hbm": bytes_ / (ms * 1e-3) / 1e9 / hbm,
-                        "frac_of_8TBps": bytes_ / (ms * 1e-3) / 1e9 / 8000.0,
+                        "frac_of_datasheet_hbm": bytes_ / (ms * 1e-3) / 1e9 / HBM_DATASHEET_GBS,
                         "kernel_ms": {"rowstats": kms[0], "lattice": kms[1], "grad": kms[2],
                                       "note": ("this shape runs as 4 overlapped batch groups (a group's wavefront on a side stream beside "
                                                "the streaming passes of the others): rowstats = pass 1 of all groups with the co-running "
                                                "wavefronts, lattice = only the exposed wait before the first pass 2, grad = pass 2 of all "
-                                               "groups; the whole kernels alone (RNNT_B200_GROUPS=1) are in profiles/r2_c4_full.md")
+                                               "groups; RNNT_B200_GROUPS=1 times the whole kernels alone")
                                       if key == "c4" else "separate pass with event markers between the kernels (no launch overlap)"},
                         "l2": "flushed before every step" if small else "inputs exceed L2"}
             del sh
@@ -532,6 +543,18 @@ def other_workloads_leg(torch, wr, dev, peaks):
     return out
 
 
+def dump_outputs(out_dir, costs, grads):
+    """What the caller of the timed path receives from its last step (see the module docstring)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    c = costs.float().cpu().numpy()
+    idx = np.sort(np.random.default_rng(DUMP_SEED).integers(0, grads.numel(), size=min(DUMP_SAMPLES, grads.numel())))
+    g = grads.view(-1)[torch.as_tensor(idx, device=grads.device)].float().cpu().numpy()
+    np.save(os.path.join(out_dir, "costs.npy"), c)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([c.sum(dtype=np.float64)], np.float32))
+    np.save(os.path.join(out_dir, "grads_sample.npy"), g)
+
+
 # ----------------------------------------------------------------------------------------------
 # Our arm
 # ----------------------------------------------------------------------------------------------
@@ -545,7 +568,7 @@ def run_b200_arm(args):
     import warprnnt_pytorch.warp_rnnt as wr
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 arm has no CPU fallback)")
+        raise SystemExit("bench.py: no CUDA device (the GPU arm has no CPU fallback)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -622,8 +645,10 @@ def run_b200_arm(args):
         del flush
     launches = wr.last_launch_count() * args.steps
     wr.set_profiling(False)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, costs, grads)
 
-    # ---- secondary, reported separately (SURVEY 8(d)): ragged lengths ~U[0.5,1]*max, seed 2.
+    # ---- secondary, reported separately: ragged lengths ~U[0.5,1]*max, seed 2.
     # Padded cells are not read (pass 1 skips them, pass 2 writes zeros), so bytes move less.
     ragged = None
     try:
@@ -639,7 +664,7 @@ def run_b200_arm(args):
     except Exception as ex:
         ragged = {"error": repr(ex)[:200]}
 
-    # ---- parity on every rank (VERDICT r1: multi-GPU correctness had no driver-side evidence)
+    # ---- parity on every rank: multi-GPU correctness is checked where it runs
     parity_local = parity_leg(torch, dist, wr, sh, world, rank, dev)
 
     # ---- end to end through compute_rnnt_loss(): pinned host inputs -> device, costs -> host.
@@ -732,21 +757,14 @@ def run_b200_arm(args):
         "bound": "hbm", "kernel": "grad_row_kernel (pass 2: read logits 4 B + write gradient 4 B per element)",
         "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
         "frac": achieved / peaks["hbm_gbs"] if achieved else None, "peak_source": peak_src + " (MEASURED_PEAKS.json hbm_gbs)",
-        "traffic": None, "traffic_source": "profiles/traffic.json (ncu --set full capture of the same kernel, committed; not re-measured per run)",
         "ms_per_launch": grad_ms,
-        "frac_of_8TBps": achieved / 8000.0 if achieved else None,
+        "frac_of_datasheet_hbm": achieved / HBM_DATASHEET_GBS if achieved else None,
         "other_kernels": {
             "rowstats_row_kernel": {"ms": rows_ms, "algorithmic_GBps": 4.0 * E / (rows_ms * 1e-3) / 1e9 if rows_ms > 0 else None},
             "lattice_kernel": {"ms": lat_ms, "bound": "latency"},
             "path_12B_per_elt_GBps": 12.0 * E / ((rows_ms + lat_ms + grad_ms) * 1e-3) / 1e9 if grad_ms > 0 else None,
         },
     }
-    traffic_file = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(traffic_file):
-        try:
-            roofline["traffic"] = json.load(open(traffic_file)).get("grad_kernel_c3_bytes")
-        except Exception:
-            pass
 
     # ---- BASELINE config 5 as written, on every world size (frees the headline buffers first)
     del acts, grads, ws, sh
@@ -826,6 +844,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-c5", action="store_true", help="skip the config-5 strong-scaling leg")
     ap.add_argument("--quick", action="store_true", help="skip the reference-GPU and other-workload legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference_arm(args)
@@ -839,7 +858,8 @@ def main():
                    "--master-port", os.environ.get("MASTER_PORT", "29517"), os.path.abspath(__file__),
                    "--gpus", str(args.gpus), "--steps", str(args.steps), "--warmup", str(args.warmup),
                    "--workload", args.workload] + (["--no-cpu-baseline"] if args.no_cpu_baseline else []) + \
-                  (["--no-c5"] if args.no_c5 else []) + (["--quick"] if args.quick else [])
+                  (["--no-c5"] if args.no_c5 else []) + (["--quick"] if args.quick else []) + \
+                  (["--dump-outputs", args.dump_outputs] if args.dump_outputs else [])
             raise SystemExit(subprocess.call(cmd))
         run_b200_arm(args)
 

@@ -1,5 +1,5 @@
 /*
- * rnnt.h — C-ABI of the B200-native RNN-Transducer loss (libwarprnnt.so).
+ * rnnt.h — C-ABI of the H100-native (sm_90a) RNN-Transducer loss (libwarprnnt.so).
  *
  * Binary drop-in for the reference library's interface: the same five exported symbols, the
  * same enum values and the same 32-byte by-value options struct, so anything that links the
@@ -279,7 +279,7 @@ int rnnt_b200_profile_collect(float* ms3_mean);
  *   5  split-K slabs of the additive joint's S product for alphabet size a.   Returns -1 for an unknown `what`. */
 int rnnt_b200_debug_policy(int what, int a, int b);
 
-/* Build identification string, e.g. "b200-rnnt sm_100a <date>". */
+/* Build identification string, e.g. "b200-rnnt sm_90a <date>". */
 const char* rnnt_b200_build_info(void);
 
 #ifdef __cplusplus

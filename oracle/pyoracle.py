@@ -6,7 +6,7 @@ legs may import this module; the product package never does.
 Two checkers live behind it:
   * ``oracle/librnnt_oracle.so``         our C restatement (oracle/rnnt_oracle.c)
   * ``oracle/_ref/libwarprnnt_ref_cpu.so``  the unmodified reference CPU path, compiled
-    from /root/reference by oracle/Makefile (prebuilt file travels to the GPU box)
+    by oracle/Makefile where the reference sources are present (optional)
 """
 import ctypes as C
 import os
@@ -173,6 +173,80 @@ def ref_cpu_logprobs(log_probs, labels, act_lens, label_lens, blank=0, want_grad
     if rc != 0:
         raise RuntimeError("reference compute_rnnt_loss rc=%d" % rc)
     return costs, grads
+
+
+# --------------------------------------------------------------------------------------
+# Fixed inputs of the stored reference answers (tests/golden/make_golden.py writes them,
+# the tests recompute the inputs and compare against the stored outputs).
+# --------------------------------------------------------------------------------------
+def det_uniform(shape, seed, device):
+    """float32 values in [0, 1) from an integer hash of (flat index, seed): the same numbers on every
+    device, driver and torch version, unlike a torch generator whose stream follows the launch grid."""
+    import torch
+    n = int(np.prod(shape))
+    out = torch.empty(n, dtype=torch.float32, device=device)
+    step = 1 << 26
+    for s in range(0, n, step):
+        x = torch.arange(s, min(n, s + step), dtype=torch.int64, device=device)
+        x = (x + seed * 0x632BE5AB) & 0xFFFFFFFF
+        x = (((x >> 16) ^ x) * 0x45D9F3B) & 0xFFFFFFFF
+        x = (((x >> 16) ^ x) * 0x45D9F3B) & 0xFFFFFFFF
+        x = (x >> 16) ^ x
+        out[s:s + x.numel()] = (x >> 8).to(torch.float32) * (1.0 / (1 << 24))
+    return out.view(*shape)
+
+
+# name: (N, T, L, V, ragged lengths, seed) - the README shapes of the reference and the headline shape
+REF_GPU_CASES = {
+    "small": (8, 50, 10, 15, True, 5),
+    "readme_small_vocab": (16, 150, 40, 28, True, 5),
+    "readme_large_vocab_N4": (4, 150, 20, 5000, True, 5),
+    "headline": (128, 150, 20, 5000, False, 9),
+}
+GRAD_SAMPLES = 512   # gradient elements stored per case, at seeded positions
+
+
+def ref_gpu_case_inputs(name, device):
+    """(acts [N,T,U,V] on `device`, labels, act_lens, label_lens, sampled flat gradient indices)."""
+    N, T, L, V, ragged, seed = REF_GPU_CASES[name]
+    acts = det_uniform((N, T, L + 1, V), seed, device)
+    rng = np.random.default_rng(seed)
+    labels = rng.integers(1, V, size=(N, L)).astype(np.int32)
+    tl, ul = np.full(N, T, np.int32), np.full(N, L, np.int32)
+    if ragged:
+        tl[1::3] = rng.integers(T // 2, T + 1, size=len(tl[1::3]))
+        ul[2::3] = rng.integers(0, L + 1, size=len(ul[2::3]))
+    idx = np.sort(rng.integers(0, acts.numel(), size=GRAD_SAMPLES, dtype=np.int64))
+    return acts, labels, tl, ul, idx
+
+
+def gpu_loss(lib, workspace_bytes, acts, labels, act_lens, label_lens, opt_type):
+    """compute_rnnt_loss(loc=GPU) of a C-ABI library `lib` (this project's or the reference's) on device
+    tensors; returns (costs as numpy float32, gradient tensor pre-filled with NaN)."""
+    import torch
+    dev = acts.device
+    N, T, U, V = acts.shape
+    lab, tl, ul = (torch.as_tensor(x).to(dev) for x in (labels, act_lens, label_lens))
+    opt = opt_type(loc=1, num_threads=0, stream=torch.cuda.current_stream(dev).cuda_stream,
+                   blank_label=0, maxT=T, maxU=U, batch_first=True)
+    ws = torch.empty(workspace_bytes, dtype=torch.uint8, device=dev)
+    grads = torch.full_like(acts, float("nan"))
+    costs = np.zeros(N, np.float32)
+    st = lib.compute_rnnt_loss(acts.data_ptr(), grads.data_ptr(), lab.data_ptr(), ul.data_ptr(),
+                               tl.data_ptr(), V, N, costs.ctypes.data, ws.data_ptr(), opt)
+    if st != 0:
+        raise RuntimeError("compute_rnnt_loss status %d" % st)
+    torch.cuda.synchronize(dev)
+    return costs, grads
+
+
+def grad_summary(grads, idx):
+    """(gradient values at the flat positions idx, per-utterance sum of squares in float64)."""
+    import torch
+    flat = grads.view(-1)
+    at = flat[torch.as_tensor(idx, device=grads.device)].cpu().numpy()
+    sumsq = np.array([float((grads[b].double() ** 2).sum()) for b in range(grads.shape[0])])
+    return at, sumsq
 
 
 def log_softmax_np(x):

@@ -1,7 +1,11 @@
 #!/usr/bin/env python
-"""Regenerates the committed golden fixtures.  Runs ONLY in the authoring container
-(needs /root/reference and oracle/_ref built by oracle/Makefile); the GPU box and the test
-suite read the committed outputs, never the reference.
+"""Regenerates the committed golden fixtures from the reference implementation (needs the reference
+sources, $RNNT_REFERENCE, and oracle/_ref built from them by oracle/Makefile); the test suite reads the
+committed outputs, never the reference.
+
+    python tests/golden/make_golden.py                 # known_answers.json, ref_cases.npz, ref_live_cpu.npz
+    python tests/golden/make_golden.py --ref-gpu DIR   # DIR/ref_gpu_cases.npz (needs a GPU and
+                                                       # oracle/_ref/libwarprnnt_ref_gpu.so only)
 
 Outputs (next to this script):
   known_answers.json  the known-answer vectors the reference's own tests hold for this path,
@@ -11,6 +15,10 @@ Outputs (next to this script):
                         - oracle/_ref/libwarprnnt_ref_cpu.so (compiled unmodified reference CPU
                           path) composed with log_softmax fwd/bwd, fp32 and fp64
                         - pytorch_binding/test/transducer_np.py (the reference's numpy model)
+  ref_live_cpu.npz    the reference CPU library itself (log-prob and logits conventions, with and
+                      without gradients) on the seeded cases of tests/test_oracle.py
+  ref_gpu_cases.npz   the reference's own CUDA kernels on the fixed inputs of pyoracle.REF_GPU_CASES:
+                      costs, gradients at GRAD_SAMPLES seeded positions, per-utterance sums of squares
 """
 import importlib.util
 import json
@@ -111,9 +119,68 @@ def make_case(rng, N, T, U, V, blank, ragged, scale):
     return acts, labels, act_lens, label_lens
 
 
+LIVE_CPU_SHAPES = [(3, 11, 6, 10), (2, 50, 10, 15), (65, 10, 5, 5), (1, 50, 15, 20)]
+LIVE_CPU_SAMPLES = 256
+
+
+def live_cpu_case(i, rng):
+    """Case i of tests/test_oracle.py::test_against_reference_cpu_library (draws from the shared rng)."""
+    N, T, U, V = LIVE_CPU_SHAPES[i]
+    acts = rng.random((N, T, U, V), dtype=np.float32)      # U[0,1) like tests/random.cpp:13-20
+    labels = rng.integers(1, V, size=(N, U - 1)).astype(np.int32)
+    tl = rng.integers(T // 2 + 1, T + 1, size=N).astype(np.int32)
+    ul = rng.integers(0, U, size=N).astype(np.int32)
+    tl[0], ul[0] = T, U - 1
+    idx = np.sort(np.random.default_rng(100 + i).integers(0, acts.size, size=LIVE_CPU_SAMPLES))
+    return acts, labels, tl, ul, idx
+
+
+def live_cpu():
+    rng = np.random.default_rng(7)
+    blob = {}
+    for i in range(len(LIVE_CPU_SHAPES)):
+        acts, labels, tl, ul, idx = live_cpu_case(i, rng)
+        lp = pyoracle.log_softmax_np(acts)
+        c_ref, g_ref = pyoracle.ref_cpu_logprobs(lp, labels, tl, ul, 0, threads=2)
+        c_fwd, _ = pyoracle.ref_cpu_logprobs(lp, labels, tl, ul, 0, want_grad=False)
+        c64, dx64 = pyoracle.ref_cpu_logits(acts.astype(np.float64), labels, tl, ul, 0)
+        blob.update({"%d.costs" % i: c_ref, "%d.grads_at" % i: g_ref.reshape(-1)[idx],
+                     "%d.costs_fwd" % i: c_fwd, "%d.costs_f64" % i: c64,
+                     "%d.dx_f64_at" % i: dx64.reshape(-1)[idx]})
+    np.savez_compressed(os.path.join(HERE, "ref_live_cpu.npz"), **blob)
+
+
+def ref_gpu(out_dir):
+    """The reference's CUDA kernels (oracle/_ref/libwarprnnt_ref_gpu.so) on pyoracle.REF_GPU_CASES."""
+    import ctypes as C
+    import torch
+    ref = C.CDLL(pyoracle.ref_gpu_path())
+    ref.compute_rnnt_loss.restype = C.c_int
+    ref.compute_rnnt_loss.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                                         pyoracle.RnntOptions]
+    ref.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
+    dev = torch.device("cuda:0")
+    blob = {"names": np.array(sorted(pyoracle.REF_GPU_CASES))}
+    for name in sorted(pyoracle.REF_GPU_CASES):
+        acts, labels, tl, ul, idx = pyoracle.ref_gpu_case_inputs(name, dev)
+        N, T, U, V = acts.shape
+        n = C.c_size_t(0)
+        assert ref.get_workspace_size(T, U, N, True, C.byref(n), 4) == 0
+        costs, grads = pyoracle.gpu_loss(ref, n.value, acts, labels, tl, ul, pyoracle.RnntOptions)
+        at, sumsq = pyoracle.grad_summary(grads, idx)
+        blob.update({name + ".costs": costs, name + ".grads_at": at, name + ".sumsq": sumsq})
+        print("%-22s N=%d T=%d U=%d V=%d cost0=%.4f" % (name, N, T, U, V, costs[0]), flush=True)
+        del acts, grads
+        torch.cuda.empty_cache()
+    os.makedirs(out_dir, exist_ok=True)
+    np.savez_compressed(os.path.join(out_dir, "ref_gpu_cases.npz"), **blob)
+
+
 def main():
+    if "--ref-gpu" in sys.argv:
+        return ref_gpu(sys.argv[sys.argv.index("--ref-gpu") + 1])
     if not os.path.isdir(REF):
-        sys.exit("reference not present; fixtures can only be regenerated in the authoring container")
+        sys.exit("reference sources not found (set RNNT_REFERENCE)")
     pyoracle.build()
     assert pyoracle.have_ref_cpu()
     json.dump(known_answers(), open(os.path.join(HERE, "known_answers.json"), "w"), indent=1)
@@ -144,6 +211,7 @@ def main():
         })
         print("%-16s N=%d T=%d U=%d V=%d blank=%d costs=%s" % (name, N, T, U, V, blank, c64))
     np.savez_compressed(os.path.join(HERE, "ref_cases.npz"), **blob)
+    live_cpu()
     print("wrote", os.path.join(HERE, "known_answers.json"), os.path.join(HERE, "ref_cases.npz"))
 
 

@@ -1,5 +1,5 @@
 """(Manual perf script, lives under tests/ because it executes oracle/_ref; not collected by pytest.)
-Times the reference's own CUDA kernels (oracle/_ref/libwarprnnt_ref_gpu.so, compiled for sm_100)
+Times the reference's own CUDA kernels (oracle/_ref/libwarprnnt_ref_gpu.so, compiled for sm_90)
 on the BASELINE shapes — the denominator of the north-star '>= 10x the reference GPU kernel'.
 Timed like tests/test_time.cu: wall clock around compute_rnnt_loss (it synchronises), 10 calls."""
 import ctypes as C

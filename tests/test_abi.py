@@ -131,7 +131,7 @@ def test_operator_rejects_cpu_tensors_and_bad_inputs():
 
 
 def test_dispatch_policy_matches_the_design_notes(wr):
-    """Host-side shape policy (DESIGN.md 3): the values the measurements in profiles/ were taken with."""
+    """Host-side shape policy (DESIGN.md 2-4): the values the H100 measurements in DESIGN.md were taken with."""
     lib = wr.lib()
     lib.rnnt_b200_debug_policy.restype = C.c_int
     lib.rnnt_b200_debug_policy.argtypes = [C.c_int, C.c_int, C.c_int]

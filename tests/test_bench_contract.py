@@ -1,5 +1,5 @@
 """bench.py contract checks that need no GPU: the reference arm runs on the CPU and prints ONE JSON
-line with the keys the driver reads; the B200 arm refuses to run without a CUDA device."""
+line with the keys a consumer reads; the GPU arm refuses to run without a CUDA device."""
 import json
 import os
 import subprocess

@@ -38,7 +38,7 @@ def reference_style():
     grads.mul_(torch.ones(1, device=dev).view(-1, 1, 1, 1))   # backward :47-50
 
 
-for name, fn in (("warprnnt_pytorch (B200) step", ours), ("reference operator's pass structure", reference_style)):
+for name, fn in (("warprnnt_pytorch step", ours), ("reference operator's pass structure", reference_style)):
     for _ in range(3):
         fn()
     torch.cuda.synchronize()

@@ -1,9 +1,8 @@
-"""Builds libwarprnnt.so (the C-ABI drop-in) in-tree for sm_100a with nvcc.
+"""Builds libwarprnnt.so (the C-ABI drop-in) in-tree for sm_90a (H100) with nvcc.
 
     python warp-transducer_b200/build.py [--force] [--verbose]
 
-The shared object lands in warp-transducer_b200/lib/ (git-ignored, shipped to the GPU box with
-the tree).  cudart is linked statically so the library has no run-time dependency beyond the
+The shared object lands in warp-transducer_b200/lib/ (git-ignored).  cudart is linked statically so the library has no run-time dependency beyond the
 driver; it shares the primary context (and therefore streams and device pointers) with PyTorch.
 """
 import os
@@ -18,7 +17,7 @@ SOURCES = ["rnnt_entry.cu"]
 DEPS = sorted(f for f in os.listdir(SRC) if f.endswith((".cu", ".cuh", ".h"))) + \
        [os.path.join("..", "..", "include", "rnnt.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
 ]
 

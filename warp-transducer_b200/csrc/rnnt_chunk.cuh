@@ -106,9 +106,9 @@ __device__ __forceinline__ void chunk_issue(const T* __restrict__ acts, T* tile,
 // Per-row SCALAR work (index decoding, lengths, label, the statistics' logarithm, the factor split, the
 // skewed store address) is done ROW-PARALLEL: thread r of the CTA owns row r's scalars, so that work runs
 // on ROWS/32 fully populated warps instead of being repeated by (or idling) the TPR lanes that share a row.
-// At V=28 it was most of the kernel (ncu: 54 instructions per element, 87 % issue-active).
+// At small V it is most of the kernel (the loop is issue-bound).
 // The element walk is group-parallel: TPR lanes per row, results handed over through shared memory.
-// The CTA size NT is a template parameter (tuning hook; 256 measured best on B200).
+// The CTA size NT is a template parameter (tuning hook RNNT_B200_CHUNK_NT; default 256).
 // =================================================================================================
 template <typename T, int TPR, int NT>
 __global__ void __launch_bounds__(NT)
@@ -259,9 +259,8 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
 
     // Row constants: every lane fetches its row's constants itself (lanes of a row hit the same addresses, so
     // the loads coalesce into one request per row).  The row-parallel form (thread r <-> row r, hand-over
-    // through shared memory, as in pass 1) is kept behind ROWPAR: measured on B200 it is slower here - at
-    // V=28 the extra shared-memory hop behind the barrier costs more than the saved instructions (grad
-    // 43 -> 47 us), and at V=50 the hand-over array costs the eighth resident CTA per SM.
+    // through shared memory, as in pass 1) is kept behind ROWPAR: the extra shared-memory hop behind the barrier
+    // costs more than the saved instructions at small V, and the hand-over array costs resident CTAs per SM.
     constexpr bool ROWPAR = false;
     auto fetch = [&](uint32_t row_in_chunk) {
         const bool inrange = row_in_chunk < nrows;

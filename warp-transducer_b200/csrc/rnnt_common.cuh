@@ -1,4 +1,4 @@
-// rnnt_common.cuh — small device/host helpers shared by the sm_100a RNN-T kernels.
+// rnnt_common.cuh — small device/host helpers shared by the sm_90a RNN-T kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -105,7 +105,7 @@ template <> struct ExpSum<double> {
 // ---------------------------------------------------------------------------------------------
 // Vectorised global access with cache policy.  BYTES in {4, 8, 16}.
 //   ld_keep   : read-only path, normal L2 residency (first pass over the logits: on shapes that fit
-//               the 126 MB L2 the second pass then hits)
+//               the 50 MB L2 the second pass then hits)
 //   ld_stream : evict-first (second/last pass over the logits)
 //   st_stream : evict-first store (gradients are never re-read by this library)
 // ---------------------------------------------------------------------------------------------

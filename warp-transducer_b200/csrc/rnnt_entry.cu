@@ -277,7 +277,7 @@ void launch_grad_tile(const IO* acts, IO* grads, const int* labels, const int* x
 }
 
 // lanes per row for the register-tile kernels: the fewest lanes (>= 2) whose kVPL = 8 vector
-// registers hold the row - measured on B200: V=28 -> 2 lanes, V=50 (float2) -> 4 lanes per row
+// registers hold the row: V=28 -> 2 lanes, V=50 (float2) -> 4 lanes per row
 inline int pick_lpr(int nv) {
     static const int forced = [] {
         const char* e = getenv("RNNT_B200_LPR");  // tuning hook
@@ -336,7 +336,7 @@ void stream_passes(const IO* acts, IO* grads, const int* labels, const int* xlen
 // ---- short rows (<= 512 B): chunk kernels (rnnt_chunk.cuh), TMA bulk staging of R consecutive rows ----
 // Threads per row: as FEW as keep a thread's share at <= 32 elements (two for even V, so that the walk can use
 // 8-byte pairs) - every lane of a row repeats the row's fixed work (mapping, shuffles, reductions), and at
-// V = 28 that fixed work dominated: 4 lanes/row 0.099 ms, 2 lanes/row 0.079 ms for the whole C2 call.  Bank
+// V = 28 that fixed work dominates, so fewer lanes per row win.  Bank
 // conflicts are dealt with by the lane mapping (chunk_walk_cost), not by the lane count.
 // RNNT_B200_CHUNK=0 routes short rows to the register-tile kernels.
 inline int pick_tpr(int V) {
@@ -605,16 +605,15 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
     };
 
     // Overlap decision: the wavefront costs ~0.25 us per anti-diagonal whatever the batch; the
-    // streaming passes cost 12 B/elt at ~6.9 TB/s.  Worth splitting only when the lattice is a
-    // visible share of a call that is long enough to amortise the extra launches.
-    // Measured on B200 (N=64,T=1500,U=301,V=50): 3.88 -> 3.77 ms with 4 groups; the co-running
-    // lattice CTAs slow the streaming kernels a little, so the gain is modest, and there is none
+    // streaming passes cost 12 B/elt at ~3.0 TB/s (what they reach on an H100 SXM).  Worth splitting only
+    // when the lattice is a visible share of a call that is long enough to amortise the extra launches.
+    // The co-running lattice CTAs slow the streaming kernels a little, so the gain is modest, and there is none
     // when no pass 2 follows in the same call (loss-only / operator forward) - those stay in order.
     int groups = 1;
     if (phase == kFull && grads && N >= 2 * kAutoGroups && !d.tmajor) {
         static const int forced = [] { const char* e = getenv("RNNT_B200_GROUPS"); return e ? atoi(e) : 0; }();
         const double lattice_us = 0.25 * (opt.maxT + opt.maxU) + 20.0;
-        const double stream_us = (double)rows64 * V * sizeof(IO) * (grads ? 3.0 : 1.0) / 6.9e6;
+        const double stream_us = (double)rows64 * V * sizeof(IO) * (grads ? 3.0 : 1.0) / 3.0e6;
         if (stream_us > 400.0 && lattice_us > 0.08 * stream_us) groups = kAutoGroups;
         if (forced >= 1 && forced <= kMaxGroups && forced <= N) groups = forced;
         if (groups > 1 && !side_pool().ok) groups = 1;
@@ -625,9 +624,8 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
     // EXPERIMENTAL, off unless RNNT_B200_PDL=1: launch the lattice and gradient kernels with programmatic
     // stream serialization, so their prologues (and the gradient kernel's first wave of logit loads) overlap
     // the tail of the kernel before them; each waits (griddepcontrol.wait) before it touches that kernel's
-    // output.  Measured on B200: C2 0.128 vs 0.130 ms, C3/C4 unchanged - the three kernels are each bound by
-    // their own latency chains, not by the launch gaps - and one 16-bit parity case differed, so it stays
-    // opt-in.  (The event markers of the profiling mode would serialise the kernels anyway.)
+    // output.  The three kernels are each bound by their own latency chains rather than by the launch gaps,
+    // so it stays opt-in.  (The event markers of the profiling mode would serialise the kernels anyway.)
     static const bool pdl_env = [] { const char* e = getenv("RNNT_B200_PDL"); return e && atoi(e) != 0; }();
     g_pdl = pdl_env && groups == 1 && !g_profile;
     if (groups == 1) {
@@ -731,7 +729,7 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
     w.mf = static_cast<float*>(take((size_t)N * T * 4));
     w.mg = static_cast<float*>(take((size_t)N * U * 4));
     w.inv_s = static_cast<float*>(take(C * 4));
-    w.wm = static_cast<float*>(take(std::max(C, (size_t)N * T * umma::kWmPad) * 4));   // rows padded for the fused gradient kernel
+    w.wm = static_cast<float*>(take(std::max(C, (size_t)N * T * wg::kWmPad) * 4));   // rows padded for the fused gradient kernel
     w.bk = static_cast<float*>(take(C * 4));
     w.lb = static_cast<float*>(take(C * 4));
     w.part = static_cast<float*>(take(C * 4 * kJointSlices));
@@ -744,25 +742,24 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
     return w;
 }
 
-// ---- tensor-core contractions of the additive joint (rnnt_umma.cuh) ---------------------------------
-// N (accumulator columns per CTA) is the smallest instantiated width that holds `n`, tiled beyond 256.
-inline bool joint_umma_enabled() {
+// ---- tensor-core contractions of the additive joint (rnnt_wgmma.cuh) ---------------------------------
+// N (accumulator columns per CTA) is the smallest instantiated width that holds `n`, tiled beyond 128
+// (a thread holds N/2 accumulators: 128 columns keep two CTAs of 256 threads resident per SM).
+inline bool joint_tc_enabled() {
     static const bool on = [] { const char* e = getenv("RNNT_B200_JOINT_SIMT"); return !(e && atoi(e) != 0); }();
     return on;
 }
 template <int A_MODE, int B_MODE, int KS>
-void launch_umma(const umma::Operand& A, const umma::Operand& B, int m, int n, int K, int slices, int batch,
-                 const umma::Epilogue& epi, cudaStream_t s, int max_tile = 256) {
+void launch_wgmma(const wg::Operand& A, const wg::Operand& B, int m, int n, int K, int slices, int batch,
+                 const wg::Epilogue& epi, cudaStream_t s, int max_tile = 128) {
     auto go = [&](auto kernel, int NT, size_t smem) {
         func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         dim3 grid((unsigned)(slices * ((n + NT - 1) / NT)), (unsigned)((m + 127) / 128), (unsigned)batch);
-        kernel<<<grid, umma::kThreads, smem, s>>>(A, B, K, slices, epi);
+        kernel<<<grid, wg::kThreads, smem, s>>>(A, B, K, slices, epi);
     };
-    if (n <= 32) go(umma::gemm_kernel<A_MODE, B_MODE, 32, KS>, 32, umma::gemm_smem_bytes<32, KS>());
-    else if (n <= 64 || max_tile <= 64) go(umma::gemm_kernel<A_MODE, B_MODE, 64, KS>, 64, umma::gemm_smem_bytes<64, KS>());
-    else if (n <= 128) go(umma::gemm_kernel<A_MODE, B_MODE, 128, KS>, 128, umma::gemm_smem_bytes<128, KS>());
-    else if (n <= 192) go(umma::gemm_kernel<A_MODE, B_MODE, 192, KS>, 192, umma::gemm_smem_bytes<192, KS>());
-    else go(umma::gemm_kernel<A_MODE, B_MODE, 256, KS>, 256, umma::gemm_smem_bytes<256, KS>());
+    if (n <= 32) go(wg::gemm_kernel<A_MODE, B_MODE, 32, KS>, 32, wg::gemm_smem_bytes<32, KS>());
+    else if (n <= 64 || max_tile <= 64) go(wg::gemm_kernel<A_MODE, B_MODE, 64, KS>, 64, wg::gemm_smem_bytes<64, KS>());
+    else go(wg::gemm_kernel<A_MODE, B_MODE, 128, KS>, 128, wg::gemm_smem_bytes<128, KS>());
 }
 
 rnntStatus_t run_add_joint(const float* f, const float* g, float* dF, float* dG, const int* labels,
@@ -815,16 +812,16 @@ rnntStatus_t run_add_joint(const float* f, const float* g, float* dF, float* dG,
     // J2: S = Ef . Eg^T in kJointSlices deterministic K-slabs, then lse + lattice log-prob pairs
     {
         const int slices = joint_slices(V);
-        if (joint_umma_enabled()) {
-            // tcgen05: M = t (tiles of 128), N = u, K = v split into `slices` slabs
-            umma::Operand A{w.ef, (long long)T * V, V, 1, T}, B{w.eg, (long long)U * V, V, 1, U};
+        if (joint_tc_enabled()) {
+            // wgmma: M = t (tiles of 128), N = u, K = v split into `slices` slabs
+            wg::Operand A{w.ef, (long long)T * V, V, 1, T}, B{w.eg, (long long)U * V, V, 1, U};
             // float4 operand fetches when every row of Ef / Eg starts on a 16-byte boundary
             // partial sums of slice ks land in slab ks: part[ks][b][t][u]
-            const umma::Epilogue epi{nullptr, 0, 0, 0, w.part, (long long)rows64, (long long)T * U, U, 1};
+            const wg::Epilogue epi{nullptr, 0, 0, 0, w.part, (long long)rows64, (long long)T * U, U, 1};
             if (V % 4 == 0)
-                launch_umma<2, 2, 32>(A, B, T, U, V, slices, N, epi, s);
+                launch_wgmma<2, 2, 32>(A, B, T, U, V, slices, N, epi, s);
             else
-                launch_umma<1, 1, 32>(A, B, T, U, V, slices, N, epi, s);
+                launch_wgmma<1, 1, 32>(A, B, T, U, V, slices, N, epi, s);
         } else {
             Operand A{w.ef, (size_t)T * V, V, 1}, B{w.eg, (size_t)U * V, V, 1};
             dim3 grid((U + 63) / 64, (T + 63) / 64, N * slices);
@@ -858,40 +855,40 @@ rnntStatus_t run_add_joint(const float* f, const float* g, float* dF, float* dG,
     }  // phase != kBackward
     if (want_grad) {
         static const bool fused = [] { const char* e = getenv("RNNT_B200_JOINT_FUSED"); return !(e && atoi(e) == 0); }();
-        const bool use_fused = fused && joint_umma_enabled() && U <= umma::kWmPad &&
-                               (uint64_t)N * T * umma::kWmPad < (1ull << 31);   // padded weights are indexed with 32 bits
-        const int wm_pitch = use_fused ? umma::kWmPad : U;
+        const bool use_fused = fused && joint_tc_enabled() && U <= wg::kWmPad &&
+                               (uint64_t)N * T * wg::kWmPad < (1ull << 31);   // padded weights are indexed with 32 bits
+        const int wm_pitch = use_fused ? wg::kWmPad : U;
         const unsigned wm_entries = (unsigned)N * T * wm_pitch;
         joint_weights_kernel<<<(wm_entries + 255) / 256, 256, 0, s>>>(w.lp2, w.alphas, w.betas, w.llf, w.inv_s, xlen, ylen,
                                                                      w.wm, w.bk, w.lb, scale, scale_vec, d, wm_pitch);
-        if (joint_umma_enabled()) {
-            // tcgen05, vocabulary index on the accumulator lanes (coalesced epilogue):
+        if (joint_tc_enabled()) {
+            // wgmma, vocabulary index on the accumulator rows (32-byte sectors in the epilogue):
             //   dF[t,v] = Ef[t,v] * sum_u Eg[u,v] Wm[t,u]      M = v, N = t, K = u
             //   dG[u,v] = Eg[u,v] * sum_t Ef[t,v] Wm[t,u]      M = v, N = u, K = t
-            umma::Operand EgT{w.eg, (long long)U * V, 1, V, V}, EfT{w.ef, (long long)T * V, 1, V, V};
-            umma::Operand WmTU{w.wm, (long long)T * U, U, 1, T};   // (n = t, k = u): k-contiguous
-            umma::Operand WmUT{w.wm, (long long)T * U, 1, U, U};   // (n = u, k = t): n-contiguous
-            // 64-column accumulator tiles: small tensor-memory / shared-memory footprint -> several CTAs per SM,
+            wg::Operand EgT{w.eg, (long long)U * V, 1, V, V}, EfT{w.ef, (long long)T * V, 1, V, V};
+            wg::Operand WmTU{w.wm, (long long)T * U, U, 1, T};   // (n = t, k = u): k-contiguous
+            wg::Operand WmUT{w.wm, (long long)T * U, 1, U, U};   // (n = u, k = t): n-contiguous
+            // 64-column accumulator tiles: small register / shared-memory footprint -> several CTAs per SM,
             // and the whole tile's Ef fetches are in flight before the accumulator is read
             static const int df_tile = [] { const char* e = getenv("RNNT_B200_DF_TILE"); return e ? atoi(e) : 64; }();
             if (use_fused) {
-                // both contractions in one pass over Ef (rnnt_umma.cuh: grad_fused_kernel)
-                const umma::GradFused gf{w.ef, w.eg, w.wm, dF, dG, T, U, V};
+                // both contractions in one pass over Ef (rnnt_wgmma.cuh: grad_fused_kernel)
+                const wg::GradFused gf{w.ef, w.eg, w.wm, dF, dG, T, U, V};
                 static const size_t pad = [] { const char* e = getenv("RNNT_B200_FUSED_PAD_SMEM"); return e ? (size_t)atoi(e) : (size_t)0; }();
-                const size_t smem = umma::GradFusedGeom<32, 32>::total + pad;   // pad: residency experiment hook
+                const size_t smem = wg::GradFusedGeom<32, 32>::total + pad;   // pad: residency experiment hook
                 auto go = [&](auto kernel) {
                     func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                    kernel<<<dim3((unsigned)((V + 127) / 128), 1, (unsigned)N), umma::kThreads, smem, s>>>(gf);
+                    kernel<<<dim3((unsigned)((V + 127) / 128), 1, (unsigned)N), wg::kThreads, smem, s>>>(gf);
                 };
-                if (V % 4 == 0) go(umma::grad_fused_kernel<32, 32, 3>);
-                else go(umma::grad_fused_kernel<32, 32, 0>);
+                if (V % 4 == 0) go(wg::grad_fused_kernel<32, 32, 3>);
+                else go(wg::grad_fused_kernel<32, 32, 0>);
             } else {
-            const umma::Epilogue epf{w.ef, (long long)T * V, 1, V, dF, 0, (long long)T * V, 1, V};
-            if (V % 4 == 0) launch_umma<3, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, df_tile);   // 16-byte aligned rows
-            else launch_umma<0, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, df_tile);
-            const umma::Epilogue epg{w.eg, (long long)U * V, 1, V, dG, 0, (long long)U * V, 1, V};
-            if (V % 4 == 0) launch_umma<3, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
-            else launch_umma<0, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
+            const wg::Epilogue epf{w.ef, (long long)T * V, 1, V, dF, 0, (long long)T * V, 1, V};
+            if (V % 4 == 0) launch_wgmma<3, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, df_tile);   // 16-byte aligned rows
+            else launch_wgmma<0, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, df_tile);
+            const wg::Epilogue epg{w.eg, (long long)U * V, 1, V, dG, 0, (long long)U * V, 1, V};
+            if (V % 4 == 0) launch_wgmma<3, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
+            else launch_wgmma<0, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
             }
         } else if (V >= 512) {  // long vocabulary: one thread per column, thin contraction
             {   // dF[t,v] = Ef[t,v] * sum_u Wm[t,u] Eg[u,v]
@@ -1227,6 +1224,6 @@ int rnnt_b200_debug_policy(int what, int a, int b) {
     }
 }
 
-const char* rnnt_b200_build_info(void) { return "b200-rnnt sm_100a built " __DATE__ " " __TIME__; }
+const char* rnnt_b200_build_info(void) { return "b200-rnnt sm_90a built " __DATE__ " " __TIME__; }
 
 }  // extern "C"

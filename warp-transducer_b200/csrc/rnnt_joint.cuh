@@ -19,7 +19,7 @@
 #pragma once
 #include "rnnt_kernels.cuh"
 #include "rnnt_lattice.cuh"
-#include "rnnt_umma.cuh"
+#include "rnnt_wgmma.cuh"
 
 namespace b200rnnt {
 

@@ -1,4 +1,4 @@
-// rnnt_kernels.cuh — the three sm_100a kernels of the RNN-T loss + gradient path (each streaming
+// rnnt_kernels.cuh — the three sm_90a kernels of the RNN-T loss + gradient path (each streaming
 // pass comes as a CTA-per-row kernel for long rows and a register-tile kernel for short rows).
 //
 //   rowstats_*       pass 1 over the logits [N,T,U,V]: per lattice cell the log-softmax statistics
@@ -68,9 +68,9 @@ __device__ __forceinline__ void utt_extent(const Dims& d, const int* __restrict_
 
 // =================================================================================================
 // Pass 1, long rows: ONE CTA PER ROW, non-persistent grid (grid = N*T*U blocks of 256 threads).
-// Measured on B200 (tools/probe/bw_probe.cu): a short-lived block that issues all its loads and
-// retires streams 8 GB at 7.5 TB/s, a persistent grid-stride loop over the same bytes at 7.1 TB/s
-// (read) / 6.0 vs 6.85 TB/s (read+write) - block turnover keeps the DRAM access window compact.
+// A short-lived block that issues all its loads and retires streams faster than a persistent grid-stride
+// loop over the same bytes (tools/probe/bw_probe.cu compares the two) - block turnover keeps the DRAM
+// access window compact.
 // Thread i owns vectors i, i+256, ... (NV per trip, all loads issued before first use; one trip
 // when V/VEC <= 256*NV, i.e. V <= 8192 in fp32).  Per trip the statistics are the exact two-pass
 // max / sum exp(x-max) from registers; trips are merged online.  Block combine: warp shuffles, one

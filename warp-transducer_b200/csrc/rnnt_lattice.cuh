@@ -2,8 +2,7 @@
 //
 // The log-domain recurrence (lattice_kernel in rnnt_kernels.cuh, kept for fp64) puts
 // SHFL -> DADD -> DADD -> F2F -> FMUL -> MUFU.EX2 -> FADD -> MUFU.LG2 -> FMUL -> F2F -> DADD on the
-// dependent chain of every anti-diagonal: ~390 cycles per step on sm_100 (round 1: 200-240 ns per
-// diagonal whatever the batch).  Here a lattice value is  v * 2^e  with v a float in [1,2) and e an
+// dependent chain of every anti-diagonal, and that chain, not the batch, sets the time per diagonal.  Here a lattice value is  v * 2^e  with v a float in [1,2) and e an
 // int, and a transition probability is  m * 2^k  (m in [0.71,1.42], k int), both prepared by pass 1:
 //
 //   product   v*m, e+k                                         FMUL || IADD          (4 cycles)
@@ -372,10 +371,9 @@ lattice_lin_kernel(const float4* __restrict__ fac, const int* __restrict__ xlen,
         lattice_lin_body<COLS, MULTI, true, RD>(fac, xlen, ylen, betas, llb, costs, d, ring_base, edge_base, prog_base, delay_base, &bad_any);
 }
 
-// Columns per lane for a label extent.  Measured on B200: a lone warp issues one instruction every 3-4
-// cycles whatever the instruction-level parallelism, so a warp-step costs ~4 cycles x its instruction count:
-//   U = 41 : 2 warps x 1 column (with the cross-warp exchange) 41 us,  1 warp x 2 columns 26 us
-//   U = 301: 10 warps x 1 column 0.43 ms,  3 warps x 4 columns 0.51 ms
+// Columns per lane for a label extent.  A lone warp issues about one instruction every few cycles whatever
+// the instruction-level parallelism, so a warp-step costs in proportion to its instruction count: two columns
+// per lane win where they remove the cross-warp exchange, while fewer, fatter warps lose at large U.
 // -> two columns per lane exactly where that saves the exchange (33..64 labels), one column otherwise.
 inline int lattice_cols(int maxU) { return maxU > 32 && maxU <= 64 ? 2 : 1; }
 inline int lattice_threads(int maxU) {

@@ -1,4 +1,4 @@
-"""warprnnt_pytorch — RNN-T loss operator for PyTorch on the B200-native libwarprnnt.
+"""warprnnt_pytorch — RNN-T loss operator for PyTorch on the H100-native libwarprnnt.
 
 Same public surface as the reference package (pytorch_binding/warprnnt_pytorch/__init__.py):
 ``RNNTLoss(blank=0, reduction='mean')``, ``rnnt_loss(acts, labels, act_lens, label_lens,
@@ -34,7 +34,7 @@ class _RNNT(Function):
         """
         length_check = certify_inputs(acts, labels, act_lens, label_lens, defer=True)
         if not acts.is_cuda:
-            raise RuntimeError("warprnnt_pytorch (B200 build) runs on CUDA tensors only; "
+            raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only; "
                                "there is no CPU fallback")
         warp_rnnt.require_same_device(acts, labels=labels, act_lens=act_lens, label_lens=label_lens)
         if reduction not in ('none', 'sum', 'mean'):

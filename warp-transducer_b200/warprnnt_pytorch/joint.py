@@ -97,7 +97,7 @@ class _AddJointRNNT(Function):
     def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction):
         length_check = certify_joint_inputs(trans, pred, labels, act_lens, label_lens, defer=True)
         if not trans.is_cuda:
-            raise RuntimeError("warprnnt_pytorch (B200 build) runs on CUDA tensors only")
+            raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only")
         warp_rnnt.require_same_device(trans, pred=pred, labels=labels, act_lens=act_lens, label_lens=label_lens)
         if reduction not in ('none', 'sum', 'mean'):
             raise ValueError("reduction must be 'none', 'sum' or 'mean'")
