@@ -224,6 +224,53 @@ rnntStatus_t rnnt_b200_backward_16(int dtype, const void* activations, void* gra
                                    struct rnntOptions options);
 
 /*
+ * Gradient regularisers, passed BY VALUE to the *_ex entries below.  Zero-initialised = both off, and the
+ * *_ex entries then launch exactly the kernels of their plain counterparts.  Both act on the gradient
+ * only: costs are the plain negative log-likelihood for every setting, bitwise identical to the costs
+ * without options (other implementations differ on what they report here).
+ *
+ *   fastemit_lambda  FastEmit (Yu et al., ICASSP 2021): the gradient with respect to the label
+ *                    log-probabilities is scaled by (1 + lambda).  Per valid cell, with p = softmax(logits),
+ *                    e_b / e_y the blank / label transition occupancies and occ = e_b + e_y:
+ *                      g_k = p_k (occ + lambda e_y) - [k = blank] e_b - [k = y_u] (1 + lambda) e_y
+ *                    This is the gradient of -ll - lambda sum_{t,u} sg[e_y] log p_y (sg = stop-gradient),
+ *                    NOT the gradient of the returned cost.  Must be finite and >= 0; 0 = off.
+ *   clamp            c > 0: every element of the per-utterance gradient is clipped to [-c, c] after the
+ *                    blank / label terms and before grad_scale * grad_costs[b]; c <= 0 = off.  Not NaN.
+ * Invalid values return RNNT_STATUS_INVALID_VALUE before any device access.
+ */
+struct rnntGradOptions {
+    float fastemit_lambda;   /* float for every storage type: fp64 calls see the options rounded to float */
+    float clamp;
+};
+#ifndef __cplusplus
+typedef struct rnntGradOptions rnntGradOptions;
+#endif
+
+/* Storage type codes of the *_ex entries (RNNT_B200_BF16 / _FP16 above are the same codes). */
+enum { RNNT_B200_FP32 = 0, RNNT_B200_FP64 = 3 };
+
+/*
+ * Full call with gradient options: dtype RNNT_B200_FP32 / _FP64 / _BF16 / _FP16, layout RNNT_B200_LAYOUT_NTUV
+ * or (fp32 / fp64 only) _TUNV.  Otherwise compute_rnnt_loss_async(_fp64), rnnt_b200_loss_async_layout(_fp64)
+ * and rnnt_b200_loss_async_16: costs_device is double* for fp64 and float* otherwise, grad_scale is rounded
+ * to the arithmetic type.  Unsupported (dtype, layout) pairs return RNNT_STATUS_INVALID_VALUE.
+ */
+rnntStatus_t rnnt_b200_loss_async_ex(int dtype, int layout, const void* activations, void* gradients,
+                                     const int* flat_labels, const int* label_lengths,
+                                     const int* input_lengths, int alphabet_size, int minibatch,
+                                     void* costs_device, double grad_scale, struct rnntGradOptions grad_options,
+                                     void* workspace, struct rnntOptions options);
+/* Backward half of the training-step split with gradient options, for all four storage types
+ * (rnnt_b200_backward / _fp64 / _16; grad_costs_device is double* for fp64, float* otherwise). */
+rnntStatus_t rnnt_b200_backward_ex(int dtype, const void* activations, void* gradients,
+                                   const int* flat_labels, const int* label_lengths,
+                                   const int* input_lengths, int alphabet_size, int minibatch,
+                                   const void* grad_costs_device, double grad_scale,
+                                   struct rnntGradOptions grad_options, void* workspace,
+                                   struct rnntOptions options);
+
+/*
  * Additive joint network, logits never materialised (SURVEY.md §8(f).2): for models whose logits
  * are  h[b,t,u,k] = trans[b,t,k] + pred[b,u,k]  (how the reference's own timing script builds them,
  * pytorch_binding/test/test_time.py:73).  trans [minibatch,maxT,V], pred [minibatch,maxU,V];
@@ -250,6 +297,14 @@ rnntStatus_t rnnt_b200_add_joint_backward(const float* trans, const float* pred,
                                           const int* label_lengths, const int* input_lengths,
                                           int alphabet_size, int minibatch, const float* grad_costs_device,
                                           float grad_scale, void* workspace, struct rnntOptions options);
+/* The same with gradient options.  FastEmit only: the factor gradients never pass through per-logit values,
+ * so any nonzero clamp returns RNNT_STATUS_INVALID_VALUE. */
+rnntStatus_t rnnt_b200_add_joint_backward_ex(const float* trans, const float* pred, float* grad_trans,
+                                             float* grad_pred, const int* flat_labels,
+                                             const int* label_lengths, const int* input_lengths,
+                                             int alphabet_size, int minibatch, const float* grad_costs_device,
+                                             float grad_scale, struct rnntGradOptions grad_options,
+                                             void* workspace, struct rnntOptions options);
 
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug

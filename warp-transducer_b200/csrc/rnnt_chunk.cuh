@@ -230,13 +230,14 @@ template <typename T> struct __align__(16) ChunkRow {
     int pad;
 };
 
-template <typename T, int TPR, int NT, bool SCALED>
+template <typename T, int TPR, int NT, bool SCALED, bool REG = false>
 __global__ void __launch_bounds__(NT)
 grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
                   const int* __restrict__ xlen, const int* __restrict__ ylen,
                   const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
                   const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                  const T* __restrict__ scale_vec, const Dims d, const int hmajor, const uint32_t wait_ns) {
+                  const T* __restrict__ scale_vec, const Dims d, const int hmajor, const uint32_t wait_ns,
+                  const GradReg<T> reg) {
     using R = Real<T>;
     using Pair = typename R::pair;
     constexpr int ROWS = NT / TPR;
@@ -286,6 +287,9 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
                 rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
                 if (SCALED && scale_vec) c.scale = __ldg(scale_vec + b) * scale_in;
             }
+        }
+        if constexpr (REG) {
+            if (v) fastemit_fold(rg, reg, b, t, u, d);
         }
         c.m = rg.m, c.cA = rg.cA, c.cB = rg.cB, c.cL = rg.cL, c.y = rg.y;
         c.valid = v ? 1 : (inrange ? 0 : -1);   // -1: row does not exist (past the end of the tensor)
@@ -348,6 +352,7 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
                 Pair v = x2[p];
                 v.x = R::exp2(fma(v.x - g.m, (T)R::kLog2e, g.cA));
                 v.y = R::exp2(fma(v.y - g.m, (T)R::kLog2e, g.cA));
+                if (REG) v.x = clip_grad(v.x, reg.clamp), v.y = clip_grad(v.y, reg.clamp);
                 if (SCALED) v.x *= g.scale, v.y *= g.scale;
                 x2[p] = v;
             }
@@ -355,6 +360,7 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
 #pragma unroll 4
             for (int k = h; k < V; k += TPR) {
                 T e = R::exp2(fma(x[k] - g.m, (T)R::kLog2e, g.cA));
+                if (REG) e = clip_grad(e, reg.clamp);
                 if (SCALED) e *= g.scale;
                 x[k] = e;
             }
@@ -364,13 +370,29 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
     }
     __syncwarp();
     if (rvalid && h == 0) {
-        T gb = R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cB));
-        if (SCALED) gb *= g.scale;
-        x[d.blank] -= gb;
-        if (g.y >= 0) {
-            T gl = R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
-            if (SCALED) gl *= g.scale;
-            x[g.y] -= gl;
+        if constexpr (REG) {
+            // the sweep stored clip(dense) at the blank and label words; the clip belongs to the corrected
+            // value, so both words are rewritten from the dense term minus their corrections
+            T gb = R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cA)) - R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cB));
+            if (g.y == d.blank) gb -= R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
+            gb = clip_grad(gb, reg.clamp);
+            if (SCALED) gb *= g.scale;
+            x[d.blank] = gb;
+            if (g.y >= 0 && g.y != d.blank) {
+                T gl = R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cA)) - R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
+                gl = clip_grad(gl, reg.clamp);
+                if (SCALED) gl *= g.scale;
+                x[g.y] = gl;
+            }
+        } else {
+            T gb = R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cB));
+            if (SCALED) gb *= g.scale;
+            x[d.blank] -= gb;
+            if (g.y >= 0) {
+                T gl = R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
+                if (SCALED) gl *= g.scale;
+                x[g.y] -= gl;
+            }
         }
     }
     if (bulk) {

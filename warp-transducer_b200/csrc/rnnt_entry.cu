@@ -6,6 +6,7 @@
 // (alpha || beta) -> grad -> costs to host + ONE stream synchronise (sync API) / nothing (async API).
 // No memset pass, no intermediate host synchronisation.
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -241,15 +242,34 @@ void launch_rowstats_row(const IO* acts, const int* labels, const int* xlen, con
     ++g_last_launches;
 }
 
+// gradient options (include/rnnt.h rnntGradOptions): validity, on/off, and the kernels' form of them
+inline bool grad_options_valid(const rnntGradOptions& o) {
+    return std::isfinite(o.fastemit_lambda) && o.fastemit_lambda >= 0.0f && !std::isnan(o.clamp);
+}
+inline bool grad_options_on(const rnntGradOptions& o) { return o.fastemit_lambda > 0.0f || o.clamp > 0.0f; }
+template <typename T> GradReg<T> make_grad_reg(const rnntGradOptions& o, const Workspace& w) {
+    GradReg<T> r;
+    r.lp2 = static_cast<const typename Lat<T>::fac*>(w.lp2);
+    const double lam = o.fastemit_lambda;
+    r.log2_lam = lam > 0.0 ? (T)std::log2(lam) : -(T)INFINITY;
+    r.log2_1p_lam = (T)(std::log1p(lam) / std::log(2.0));
+    r.clamp = o.clamp > 0.0f ? (T)o.clamp : (T)INFINITY;
+    return r;
+}
+
 template <typename T, int VEC, int NV, typename IO>
 void launch_grad_row(const IO* acts, IO* grads, const int* labels, const int* xlen, const int* ylen,
-                     const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s) {
-    auto k = (scale != T(1) || scale_vec) ? grad_row_kernel<T, VEC, NV, true, IO>
-                                          : grad_row_kernel<T, VEC, NV, false, IO>;
+                     const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s,
+                     const rnntGradOptions& ro) {
+    const bool scaled = scale != T(1) || scale_vec;
+    auto k = grad_options_on(ro) ? (scaled ? grad_row_kernel<T, VEC, NV, true, IO, true>
+                                           : grad_row_kernel<T, VEC, NV, false, IO, true>)
+                                 : (scaled ? grad_row_kernel<T, VEC, NV, true, IO>
+                                           : grad_row_kernel<T, VEC, NV, false, IO>);
     launch_k(k, dim3(d.rows), dim3(RowThreads<IO>::value), 0, s, g_pdl, acts, grads, labels, xlen, ylen,
              static_cast<const typename Real<T>::pair*>(w.stat), static_cast<const typename Lat<T>::val*>(w.alphas),
              static_cast<const typename Lat<T>::val*>(w.betas), static_cast<const typename Lat<T>::val*>(w.llf), scale,
-             scale_vec, d);
+             scale_vec, d, make_grad_reg<T>(ro, w));
     ++g_last_launches;
 }
 
@@ -265,14 +285,18 @@ void launch_rowstats_tile(const IO* acts, const int* labels, const int* xlen, co
 
 template <typename T, int VEC, int LPR, typename IO>
 void launch_grad_tile(const IO* acts, IO* grads, const int* labels, const int* xlen, const int* ylen,
-                      const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s) {
-    auto k = (scale != T(1) || scale_vec) ? grad_tile_kernel<T, VEC, LPR, true, IO>
-                                          : grad_tile_kernel<T, VEC, LPR, false, IO>;
+                      const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s,
+                      const rnntGradOptions& ro) {
+    const bool scaled = scale != T(1) || scale_vec;
+    auto k = grad_options_on(ro) ? (scaled ? grad_tile_kernel<T, VEC, LPR, true, IO, true>
+                                           : grad_tile_kernel<T, VEC, LPR, false, IO, true>)
+                                 : (scaled ? grad_tile_kernel<T, VEC, LPR, true, IO>
+                                           : grad_tile_kernel<T, VEC, LPR, false, IO>);
     const uint64_t warps = ((uint64_t)d.rows * LPR + 31) / 32;
     launch_k(k, dim3((unsigned)((warps + 7) / 8)), dim3(256), 0, s, g_pdl, acts, grads, labels, xlen, ylen,
              static_cast<const typename Real<T>::pair*>(w.stat), static_cast<const typename Lat<T>::val*>(w.alphas),
              static_cast<const typename Lat<T>::val*>(w.betas), static_cast<const typename Lat<T>::val*>(w.llf), scale,
-             scale_vec, d);
+             scale_vec, d, make_grad_reg<T>(ro, w));
     ++g_last_launches;
 }
 
@@ -291,14 +315,15 @@ inline int pick_lpr(int nv) {
 
 template <typename T, int VEC, typename IO>
 void stream_passes(const IO* acts, IO* grads, const int* labels, const int* xlen, const int* ylen,
-                   const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass) {
+                   const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass,
+                   const rnntGradOptions& ro) {
     const int nv = d.V / VEC;
     if (nv > 32 * kVPL) {  // long rows: CTA per row; NV = vectors per thread per trip
         const int per_thread = (nv + RowThreads<IO>::value - 1) / RowThreads<IO>::value;
 #define B200_ROW(NVV)                                                                             \
     do {                                                                                          \
         if (pass == 1) launch_rowstats_row<T, VEC, NVV, IO>(acts, labels, xlen, ylen, w, d, s);       \
-        else launch_grad_row<T, VEC, NVV, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s);       \
+        else launch_grad_row<T, VEC, NVV, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, ro);       \
     } while (0)
         if (sizeof(IO) <= 4 && VEC == 16 / (int)sizeof(IO)) {  // 16-B fast paths get an exact register count
             switch (per_thread) {
@@ -321,7 +346,7 @@ void stream_passes(const IO* acts, IO* grads, const int* labels, const int* xlen
 #define B200_TILE(L)                                                                              \
     case L:                                                                                       \
         if (pass == 1) launch_rowstats_tile<T, VEC, L, IO>(acts, labels, xlen, ylen, w, d, s);        \
-        else launch_grad_tile<T, VEC, L, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s);        \
+        else launch_grad_tile<T, VEC, L, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, ro);        \
         break;
     switch (pick_lpr(nv)) {
         B200_TILE(2)
@@ -370,7 +395,8 @@ inline bool chunk_enabled() {
 }
 template <typename T>
 bool chunk_pass(const T* acts, T* grads, const int* labels, const int* xlen, const int* ylen,
-                const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass) {
+                const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass,
+                const rnntGradOptions& ro) {
     using Pair = typename Real<T>::pair;
     using Fac = typename Lat<T>::fac;
     using Val = typename Lat<T>::val;
@@ -404,14 +430,16 @@ bool chunk_pass(const T* acts, T* grads, const int* labels, const int* xlen, con
             if (pass == 1)
                 prefer_smem(rowstats_chunk_kernel<T, TPR, NT>)<<<grid, NT, smem, s>>>(
                     acts, labels, xlen, ylen, static_cast<Pair*>(w.stat), static_cast<Fac*>(w.lp2), d, hmajor, wait_ns);
-            else if (scaled)
-                launch_k(prefer_smem(grad_chunk_kernel<T, TPR, NT, true>), dim3(grid), dim3(NT), smem, s, g_pdl, acts, grads,
+            else {
+                auto k = grad_options_on(ro) ? (scaled ? grad_chunk_kernel<T, TPR, NT, true, true>
+                                                       : grad_chunk_kernel<T, TPR, NT, false, true>)
+                                             : (scaled ? grad_chunk_kernel<T, TPR, NT, true>
+                                                       : grad_chunk_kernel<T, TPR, NT, false>);
+                launch_k(prefer_smem(k), dim3(grid), dim3(NT), smem, s, g_pdl, acts, grads,
                          labels, xlen, ylen, static_cast<const Pair*>(w.stat), static_cast<const Val*>(w.alphas),
-                         static_cast<const Val*>(w.betas), static_cast<const Val*>(w.llf), scale, scale_vec, d, hmajor, wait_ns);
-            else
-                launch_k(prefer_smem(grad_chunk_kernel<T, TPR, NT, false>), dim3(grid), dim3(NT), smem, s, g_pdl, acts, grads,
-                         labels, xlen, ylen, static_cast<const Pair*>(w.stat), static_cast<const Val*>(w.alphas),
-                         static_cast<const Val*>(w.betas), static_cast<const Val*>(w.llf), scale, scale_vec, d, hmajor, wait_ns);
+                         static_cast<const Val*>(w.betas), static_cast<const Val*>(w.llf), scale, scale_vec, d, hmajor, wait_ns,
+                         make_grad_reg<T>(ro, w));
+            }
         }
     };
     auto with_rpt = [&](auto tpr_c) {
@@ -437,20 +465,21 @@ bool chunk_pass(const T* acts, T* grads, const int* labels, const int* xlen, con
 
 template <typename T, typename IO>
 void stream_pass(const IO* acts, IO* grads, const int* labels, const int* xlen, const int* ylen,
-                 const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass) {
+                 const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass,
+                 const rnntGradOptions& ro) {
     if constexpr (std::is_same<T, IO>::value) {
-        if (chunk_pass<T>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass)) return;
+        if (chunk_pass<T>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass, ro)) return;
     }
     // widest vector the row pitch and the base pointers allow (16-B vectors on the fast path)
     const uintptr_t mis = reinterpret_cast<uintptr_t>(acts) | reinterpret_cast<uintptr_t>(grads) |
                           ((uintptr_t)d.V * sizeof(IO));
     constexpr int kMaxVec = 16 / sizeof(IO);
     if (mis % 16 == 0)
-        stream_passes<T, kMaxVec, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass);
+        stream_passes<T, kMaxVec, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass, ro);
     else if (sizeof(IO) == 4 && mis % 8 == 0)
-        stream_passes<T, (sizeof(IO) == 4 ? 2 : 1), IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass);
+        stream_passes<T, (sizeof(IO) == 4 ? 2 : 1), IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass, ro);
     else
-        stream_passes<T, 1, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass);
+        stream_passes<T, 1, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass, ro);
 }
 
 // What a call does.  The reference API is FULL (stats -> lattice -> grad in one call); the
@@ -462,8 +491,10 @@ template <typename IO>
 rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, const int* xlen,
                  int V, int N, typename ComputeOf<IO>::type* costs, bool async,
                  typename ComputeOf<IO>::type scale, const typename ComputeOf<IO>::type* scale_vec,
-                 Phase phase, bool want_beta, void* workspace, rnntOptions opt) {
+                 Phase phase, bool want_beta, void* workspace, rnntOptions opt,
+                 const rnntGradOptions ro = rnntGradOptions{0.0f, 0.0f}) {
     using T = typename ComputeOf<IO>::type;  // arithmetic type (float for the 16-bit storage types)
+    if (!grad_options_valid(ro)) return RNNT_STATUS_INVALID_VALUE;
     if (acts == nullptr || labels == nullptr || ylen == nullptr || xlen == nullptr ||
         (costs == nullptr && phase != kBackward) || workspace == nullptr || V <= 0 || N <= 0 ||
         opt.maxT <= 0 || opt.maxU <= 0 || (phase == kBackward && grads == nullptr))
@@ -632,7 +663,7 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
         const Group g = make_group(0, N);
         if (phase != kBackward) {
             // pass 1: log-softmax statistics + (blank, label) log-prob gather
-            stream_pass<T, IO>(g.acts, nullptr, g.labels, g.xlen, g.ylen, g.w, scale, g.scale_vec, g.d, s, 1);
+            stream_pass<T, IO>(g.acts, nullptr, g.labels, g.xlen, g.ylen, g.w, scale, g.scale_vec, g.d, s, 1, ro);
             mark(1, s);
             // lattice: alpha (and beta when gradients are or will be wanted)
             launch_lattice(g, s);
@@ -642,7 +673,7 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
         mark(2, s);
         // pass 2: dense gradient (+ zeros on padding)
         if (grads && phase != kForward) {
-            stream_pass<T, IO>(g.acts, g.grads, g.labels, g.xlen, g.ylen, g.w, scale, g.scale_vec, g.d, s, 2);
+            stream_pass<T, IO>(g.acts, g.grads, g.labels, g.xlen, g.ylen, g.w, scale, g.scale_vec, g.d, s, 2, ro);
             mark(3, s);
         }
     } else {
@@ -661,7 +692,7 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
         // main stream: pass 1 of every group back to back; each group's lattice forks off behind it
         for (int k = 0; k < groups; ++k) {
             stream_pass<T, IO>(gs[k].acts, nullptr, gs[k].labels, gs[k].xlen, gs[k].ylen, gs[k].w, scale,
-                               gs[k].scale_vec, gs[k].d, s, 1);
+                               gs[k].scale_vec, gs[k].d, s, 1, ro);
             tl.tick("rowstats_end", k, s);
             fork_ok &= cudaEventRecord(pool.forked[k], s) == cudaSuccess;
             fork_ok &= cudaStreamWaitEvent(pool.stream[k], pool.forked[k], 0) == cudaSuccess;
@@ -678,7 +709,7 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
             tl.tick("grad_beg", k, s);
             if (grads && phase != kForward)
                 stream_pass<T, IO>(gs[k].acts, gs[k].grads, gs[k].labels, gs[k].xlen, gs[k].ylen, gs[k].w,
-                                   scale, gs[k].scale_vec, gs[k].d, s, 2);
+                                   scale, gs[k].scale_vec, gs[k].d, s, 2, ro);
             tl.tick("grad_end", k, s);
         }
         tl.dump();
@@ -765,7 +796,7 @@ void launch_wgmma(const wg::Operand& A, const wg::Operand& B, int m, int n, int 
 rnntStatus_t run_add_joint(const float* f, const float* g, float* dF, float* dG, const int* labels,
                            const int* ylen, const int* xlen, int V, int N, float* costs, float scale,
                            const float* scale_vec, Phase phase, bool want_beta, void* workspace,
-                           rnntOptions opt) {
+                           rnntOptions opt, float fastemit_lambda = 0.0f) {
     if (!f || !g || !labels || !ylen || !xlen || (!costs && phase != kBackward) || !workspace || V <= 0 ||
         N <= 0 || opt.maxT <= 0 || opt.maxU <= 0 || (dF == nullptr) != (dG == nullptr) ||
         (phase == kBackward && !dF))
@@ -859,8 +890,9 @@ rnntStatus_t run_add_joint(const float* f, const float* g, float* dF, float* dG,
                                (uint64_t)N * T * wg::kWmPad < (1ull << 31);   // padded weights are indexed with 32 bits
         const int wm_pitch = use_fused ? wg::kWmPad : U;
         const unsigned wm_entries = (unsigned)N * T * wm_pitch;
-        joint_weights_kernel<<<(wm_entries + 255) / 256, 256, 0, s>>>(w.lp2, w.alphas, w.betas, w.llf, w.inv_s, xlen, ylen,
-                                                                     w.wm, w.bk, w.lb, scale, scale_vec, d, wm_pitch);
+        auto weights = fastemit_lambda > 0.0f ? joint_weights_kernel<true> : joint_weights_kernel<false>;
+        weights<<<(wm_entries + 255) / 256, 256, 0, s>>>(w.lp2, w.alphas, w.betas, w.llf, w.inv_s, xlen, ylen, w.wm, w.bk,
+                                                         w.lb, scale, scale_vec, d, wm_pitch, fastemit_lambda);
         if (joint_tc_enabled()) {
             // wgmma, vocabulary index on the accumulator rows (32-byte sectors in the epilogue):
             //   dF[t,v] = Ef[t,v] * sum_u Eg[u,v] Wm[t,u]      M = v, N = t, K = u
@@ -1090,6 +1122,57 @@ rnntStatus_t rnnt_b200_backward_16(int dtype, const void* activations, void* gra
     return RNNT_STATUS_INVALID_VALUE;
 }
 
+// ---- gradient options (FastEmit, clamp) for every storage type -------------------------------------
+rnntStatus_t rnnt_b200_loss_async_ex(int dtype, int layout, const void* activations, void* gradients,
+                                     const int* flat_labels, const int* label_lengths,
+                                     const int* input_lengths, int alphabet_size, int minibatch,
+                                     void* costs_device, double grad_scale, rnntGradOptions grad_options,
+                                     void* workspace, rnntOptions options) {
+    if (!grad_options_valid(grad_options)) return RNNT_STATUS_INVALID_VALUE;
+    if (layout != RNNT_B200_LAYOUT_NTUV && layout != RNNT_B200_LAYOUT_TUNV) return RNNT_STATUS_INVALID_VALUE;
+    const bool tunv = layout == RNNT_B200_LAYOUT_TUNV;
+    if (tunv && dtype != RNNT_B200_FP32 && dtype != RNNT_B200_FP64) return RNNT_STATUS_INVALID_VALUE;
+    auto go = [&](auto io) {
+        using IO = decltype(io);
+        using T = typename ComputeOf<IO>::type;
+        return run<IO>(static_cast<const IO*>(activations), static_cast<IO*>(gradients), flat_labels, label_lengths,
+                       input_lengths, alphabet_size, minibatch, static_cast<T*>(costs_device), true, (T)grad_scale,
+                       nullptr, kFull, false, workspace, options, grad_options);
+    };
+    g_layout_tunv = tunv;
+    rnntStatus_t st = RNNT_STATUS_INVALID_VALUE;
+    switch (dtype) {
+        case RNNT_B200_FP32: st = go(float{}); break;
+        case RNNT_B200_FP64: st = go(double{}); break;
+        case RNNT_B200_BF16: st = go(__nv_bfloat16{}); break;
+        case RNNT_B200_FP16: st = go(__half{}); break;
+    }
+    g_layout_tunv = false;
+    return st;
+}
+
+rnntStatus_t rnnt_b200_backward_ex(int dtype, const void* activations, void* gradients,
+                                   const int* flat_labels, const int* label_lengths,
+                                   const int* input_lengths, int alphabet_size, int minibatch,
+                                   const void* grad_costs_device, double grad_scale,
+                                   rnntGradOptions grad_options, void* workspace, rnntOptions options) {
+    if (!grad_options_valid(grad_options)) return RNNT_STATUS_INVALID_VALUE;
+    auto go = [&](auto io) {
+        using IO = decltype(io);
+        using T = typename ComputeOf<IO>::type;
+        return run<IO>(static_cast<const IO*>(activations), static_cast<IO*>(gradients), flat_labels, label_lengths,
+                       input_lengths, alphabet_size, minibatch, nullptr, true, (T)grad_scale,
+                       static_cast<const T*>(grad_costs_device), kBackward, false, workspace, options, grad_options);
+    };
+    switch (dtype) {
+        case RNNT_B200_FP32: return go(float{});
+        case RNNT_B200_FP64: return go(double{});
+        case RNNT_B200_BF16: return go(__nv_bfloat16{});
+        case RNNT_B200_FP16: return go(__half{});
+    }
+    return RNNT_STATUS_INVALID_VALUE;
+}
+
 // ---- additive joint network, logits never materialised -------------------------------------------
 rnntStatus_t rnnt_b200_add_joint_loss(const float* trans, const float* pred, float* grad_trans,
                                       float* grad_pred, const int* flat_labels,
@@ -1118,6 +1201,19 @@ rnntStatus_t rnnt_b200_add_joint_backward(const float* trans, const float* pred,
     return run_add_joint(trans, pred, grad_trans, grad_pred, flat_labels, label_lengths, input_lengths,
                          alphabet_size, minibatch, nullptr, grad_scale, grad_costs_device, kBackward, false,
                          workspace, options);
+}
+
+rnntStatus_t rnnt_b200_add_joint_backward_ex(const float* trans, const float* pred, float* grad_trans,
+                                             float* grad_pred, const int* flat_labels,
+                                             const int* label_lengths, const int* input_lengths,
+                                             int alphabet_size, int minibatch, const float* grad_costs_device,
+                                             float grad_scale, rnntGradOptions grad_options, void* workspace,
+                                             rnntOptions options) {
+    // the joint's gradients are contractions over weights, never per-logit values: nothing to clip
+    if (!grad_options_valid(grad_options) || grad_options.clamp != 0.0f) return RNNT_STATUS_INVALID_VALUE;
+    return run_add_joint(trans, pred, grad_trans, grad_pred, flat_labels, label_lengths, input_lengths,
+                         alphabet_size, minibatch, nullptr, grad_scale, grad_costs_device, kBackward, false,
+                         workspace, options, grad_options.fastemit_lambda);
 }
 
 rnntStatus_t rnnt_b200_add_joint_workspace_size(int maxT, int maxU, int minibatch, int alphabet_size,

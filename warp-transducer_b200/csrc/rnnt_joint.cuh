@@ -206,13 +206,15 @@ joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats ep
 
 // ---- J3: per cell weights from the lattices ---------------------------------------------------------
 //   Wm = e^{alpha+beta-ll} / S ;  Bk = blank-transition occupancy ;  Lb = label-transition occupancy
+// REG (FastEmit, rnnt_kernels.cuh GradReg): Wm += lambda Lb / S and Lb *= 1 + lambda.
+template <bool REG = false>
 __global__ void __launch_bounds__(256)
 joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
                      const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
                      const float* __restrict__ inv_s, const int* __restrict__ xlen,
                      const int* __restrict__ ylen, float* __restrict__ Wm, float* __restrict__ Bk,
                      float* __restrict__ Lb, const float scale_in, const float* __restrict__ scale_vec,
-                     const Dims d, const int wm_pitch) {
+                     const Dims d, const int wm_pitch, const float lam) {
     // Wm rows have `wm_pitch` >= maxU entries (zero beyond maxU: the tensor-core kernel fetches them as aligned
     // float4 rows); Bk / Lb / inv_s are [N,T,maxU].  One thread per Wm entry.
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -248,6 +250,10 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
             const LogVal bn = betas[q + 1];
             const float lpl2 = (float)__float_as_int(fc.w) + log2f(fc.z);
             lb = scale * exp2f((float)(oe + bn.e) + (ol + bn.l) + lpl2);
+            if (REG) {
+                w = fmaf(lam * lb, inv_s[r], w);
+                lb *= 1.0f + lam;
+            }
         }
     }
     Wm[q] = w;

@@ -3,7 +3,9 @@
 Same public surface as the reference package (pytorch_binding/warprnnt_pytorch/__init__.py):
 ``RNNTLoss(blank=0, reduction='mean')``, ``rnnt_loss(acts, labels, act_lens, label_lens,
 blank=0, reduction='mean')`` and the ``warp_rnnt`` extension functions, with the reference's
-input rules and error types (certify_inputs, :115-140).  Differences, all on the fast side:
+input rules and error types (certify_inputs, :115-140).  Keyword-only additions:
+``fastemit_lambda`` (FastEmit regularisation) and ``clamp`` (element-wise gradient clipping); see
+rnnt_loss.  Differences, all on the fast side:
 the call never synchronises with the host except for the reference's own length check, costs
 stay on the device, and the gradient is produced in autograd's backward with grad_output and the
 'mean' factor folded into the kernel - no zeros_like / mul_ passes over the [N,T,U,V] tensor.
@@ -26,12 +28,13 @@ class _RNNT(Function):
     four more full-tensor passes around its C call (zeros_like, memset, grads /= N, grads.mul_)."""
 
     @staticmethod
-    def forward(ctx, acts, labels, act_lens, label_lens, blank, reduction):
+    def forward(ctx, acts, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0, clamp=-1.0):
         """
         acts: (batch x seqLength x labelLength x outputDim) raw joint-network logits
         labels: (batch x maxLabelLength) int32 targets, zero padded
         act_lens / label_lens: (batch) int32
         """
+        warp_rnnt.grad_options(fastemit_lambda, clamp)   # ValueError before any device work
         length_check = certify_inputs(acts, labels, act_lens, label_lens, defer=True)
         if not acts.is_cuda:
             raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only; "
@@ -51,6 +54,7 @@ class _RNNT(Function):
             ctx.save_for_backward(acts, labels, act_lens, label_lens)
             ctx.workspace = ws
             ctx.blank = blank
+            ctx.fastemit_lambda, ctx.clamp = fastemit_lambda, clamp
             # reference :38-40 divides costs and grads by N for 'mean'
             ctx.scale = 1.0 / minibatch_size if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
@@ -68,30 +72,45 @@ class _RNNT(Function):
         g = g.expand(n).contiguous() if g.numel() == 1 else g.contiguous()
         grads = torch.empty_like(acts)   # the kernel defines every element (zeros on padding)
         warp_rnnt.gpu_rnnt_backward(acts, labels, act_lens, label_lens, grads, g, ctx.blank,
-                                    ctx.scale, ctx.workspace)
-        return grads, None, None, None, None, None
+                                    ctx.scale, ctx.workspace, fastemit_lambda=ctx.fastemit_lambda,
+                                    clamp=ctx.clamp)
+        return grads, None, None, None, None, None, None, None
 
 
-def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean'):
+def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean', *, fastemit_lambda=0.0,
+              clamp=-1.0):
     """RNN Transducer loss (reference :53-70).
 
     reduction: 'none' | 'sum' | 'mean'; 'mean' divides the summed loss by the batch size (what
     the reference computes, :36-40).
+
+    fastemit_lambda: FastEmit regularisation (Yu et al., ICASSP 2021), finite and >= 0; 0 = off.  The
+    gradient with respect to each label log-probability is scaled by (1 + fastemit_lambda), which
+    favours emitting labels early.  The returned loss is still the plain negative log-likelihood, so
+    with fastemit_lambda > 0 the gradient is deliberately NOT the gradient of the returned loss
+    (torch.autograd.gradcheck does not apply).
+    clamp: > 0 clips every element of each utterance's logits gradient to [-clamp, clamp], before the
+    upstream gradient and the 'mean' factor are applied (as torchaudio's rnnt_loss); <= 0 = off.
+    Invalid values raise ValueError.
     """
-    return _RNNT.apply(acts, labels, act_lens, label_lens, blank, reduction)
+    return _RNNT.apply(acts, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, clamp)
 
 
 class RNNTLoss(Module):
-    """Module form (reference :73-100): RNNTLoss(blank=0, reduction='mean')."""
+    """Module form (reference :73-100): RNNTLoss(blank=0, reduction='mean', *, fastemit_lambda=0.0,
+    clamp=-1.0); the keyword-only gradient options are those of rnnt_loss."""
 
-    def __init__(self, blank=0, reduction='mean'):
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0):
         super(RNNTLoss, self).__init__()
+        warp_rnnt.grad_options(fastemit_lambda, clamp)
         self.blank = blank
         self.reduction = reduction
+        self.fastemit_lambda, self.clamp = fastemit_lambda, clamp
         self.loss = _RNNT.apply
 
     def forward(self, acts, labels, act_lens, label_lens):
-        return self.loss(acts, labels, act_lens, label_lens, self.blank, self.reduction)
+        return self.loss(acts, labels, act_lens, label_lens, self.blank, self.reduction, self.fastemit_lambda,
+                         self.clamp)
 
 
 from ._checks import certify_inputs, check_contiguous, check_dim, check_type  # noqa: E402,F401

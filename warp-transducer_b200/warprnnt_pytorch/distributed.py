@@ -9,6 +9,7 @@ import torch
 import torch.distributed as dist
 
 from . import _RNNT, certify_inputs  # noqa: F401
+from .warp_rnnt import grad_options
 
 
 def shard_bounds(n_global, rank, world):
@@ -43,17 +44,21 @@ class ShardedRNNTLoss(torch.nn.Module):
     'sum' or 'mean' loss (identical on every rank).  backward leaves d(global loss)/d(acts) on the
     local shard.  n_global must be known up front for 'mean' (it fixes the gradient scale before
     the collective completes, so no host synchronisation is needed); pass None to infer it as
-    world_size * local batch."""
+    world_size * local batch.  fastemit_lambda / clamp: the keyword-only gradient options of rnnt_loss; the
+    clip applies to each utterance's gradient before the 1/N_global of 'mean'."""
 
-    def __init__(self, blank=0, reduction='mean', group=None, n_global=None):
+    def __init__(self, blank=0, reduction='mean', group=None, n_global=None, *, fastemit_lambda=0.0, clamp=-1.0):
         super().__init__()
+        grad_options(fastemit_lambda, clamp)
         self.blank, self.reduction, self.group, self.n_global = blank, reduction, group, n_global
+        self.fastemit_lambda, self.clamp = fastemit_lambda, clamp
 
     def forward(self, acts, labels, act_lens, label_lens):
         world = dist.get_world_size(self.group) if dist.is_initialized() else 1
         n_local = acts.size(0)
         n_global = self.n_global if self.n_global is not None else n_local * world
-        local = _RNNT.apply(acts, labels, act_lens, label_lens, self.blank, 'sum')   # [1], grads unscaled
+        local = _RNNT.apply(acts, labels, act_lens, label_lens, self.blank, 'sum', self.fastemit_lambda,
+                            self.clamp)   # [1], grads unscaled
         if self.reduction == 'mean':
             local = local / n_global            # autograd carries the 1/N_global into backward
         if world > 1:

@@ -7,7 +7,9 @@ calls RNNTLoss on the 4-D tensor; this operator takes the two factors directly:
 
 trans [N,T,V], pred [N,U,V] fp32 CUDA, same label/length conventions and input checks as RNNTLoss.
 Equivalent to RNNTLoss()(trans.unsqueeze(2) + pred.unsqueeze(1), ...) with gradients reduced to
-the factors, at O(N (T+U) V) memory traffic.
+the factors, at O(N (T+U) V) memory traffic.  The keyword-only ``fastemit_lambda`` is RNNTLoss's
+FastEmit option; ``clamp`` is not available here (the factor gradients are contractions over the
+lattice, per-logit gradients never exist to be clipped) and raises ValueError.
 """
 import ctypes as C
 
@@ -29,6 +31,9 @@ _lib.rnnt_b200_add_joint_forward.argtypes = [_P, _P, _P, _P, _P, C.c_int, C.c_in
 _lib.rnnt_b200_add_joint_backward.restype = C.c_int
 _lib.rnnt_b200_add_joint_backward.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_float, _P,
                                               warp_rnnt.rnntOptions]
+_lib.rnnt_b200_add_joint_backward_ex.restype = C.c_int
+_lib.rnnt_b200_add_joint_backward_ex.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_float,
+                                                 warp_rnnt.rnntGradOptions, _P, warp_rnnt.rnntOptions]
 _lib.rnnt_b200_add_joint_workspace_size.restype = C.c_int
 _lib.rnnt_b200_add_joint_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
 
@@ -94,7 +99,10 @@ class _AddJointRNNT(Function):
     the two factor-gradient contractions with grad_output[b] and the reduction factor folded in."""
 
     @staticmethod
-    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction):
+    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0):
+        gopt = warp_rnnt.grad_options(fastemit_lambda)   # ValueError before any device work
+        if gopt is not None:
+            gopt.clamp = 0.0                              # the joint entry accepts no clamp at all
         length_check = certify_joint_inputs(trans, pred, labels, act_lens, label_lens, defer=True)
         if not trans.is_cuda:
             raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only")
@@ -119,7 +127,7 @@ class _AddJointRNNT(Function):
         length_check.finish()   # the reference's length test, waited for with the kernels already queued
         if need:
             ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
-            ctx.ws, ctx.blank = ws, blank
+            ctx.ws, ctx.blank, ctx.gopt = ws, blank, gopt
             ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -135,23 +143,38 @@ class _AddJointRNNT(Function):
         g = g.expand(N).contiguous() if g.numel() == 1 else g.contiguous()
         dtrans, dpred = torch.empty_like(trans), torch.empty_like(pred)
         with torch.cuda.device(trans.device):
-            st = _lib.rnnt_b200_add_joint_backward(trans.data_ptr(), pred.data_ptr(), dtrans.data_ptr(),
-                                                   dpred.data_ptr(), _lab_ptr(labels), label_lens.data_ptr(),
-                                                   act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale,
-                                                   ctx.ws.data_ptr(), _joint_opts(trans, pred, ctx.blank))
+            args = (trans.data_ptr(), pred.data_ptr(), dtrans.data_ptr(), dpred.data_ptr(), _lab_ptr(labels),
+                    label_lens.data_ptr(), act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale)
+            tail = (ctx.ws.data_ptr(), _joint_opts(trans, pred, ctx.blank))
+            if ctx.gopt is not None:
+                st = _lib.rnnt_b200_add_joint_backward_ex(*args, ctx.gopt, *tail)
+            else:
+                st = _lib.rnnt_b200_add_joint_backward(*args, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_add_joint_backward failed: " + warp_rnnt.status_string(st))
-        return dtrans, dpred, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None
 
 
-def add_joint_rnnt_loss(trans, pred, labels, act_lens, label_lens, blank=0, reduction='mean'):
-    return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, blank, reduction)
+def _no_clamp(clamp):
+    if clamp is not None:
+        raise ValueError("clamp is not available for the additive joint: its factor gradients are contractions "
+                         "over the lattice and never form the per-logit gradient that clamp clips")
+
+
+def add_joint_rnnt_loss(trans, pred, labels, act_lens, label_lens, blank=0, reduction='mean', *,
+                        fastemit_lambda=0.0, clamp=None):
+    """fastemit_lambda: as rnnt_loss (the gradient is then not the gradient of the returned loss)."""
+    _no_clamp(clamp)
+    return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda)
 
 
 class AddJointRNNTLoss(Module):
-    def __init__(self, blank=0, reduction='mean'):
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=None):
         super().__init__()
-        self.blank, self.reduction = blank, reduction
+        _no_clamp(clamp)
+        warp_rnnt.grad_options(fastemit_lambda)
+        self.blank, self.reduction, self.fastemit_lambda = blank, reduction, fastemit_lambda
 
     def forward(self, trans, pred, labels, act_lens, label_lens):
-        return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, self.blank, self.reduction)
+        return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, self.blank, self.reduction,
+                                   self.fastemit_lambda)

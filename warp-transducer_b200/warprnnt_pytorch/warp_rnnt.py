@@ -8,6 +8,7 @@ The library is loaded eagerly; a missing or unloadable libwarprnnt.so is an Impo
 silent fallback.
 """
 import ctypes as C
+import math
 import os
 
 import torch
@@ -21,6 +22,11 @@ class rnntOptions(C.Structure):
     _fields_ = [("loc", C.c_int), ("num_threads", C.c_uint), ("stream", C.c_void_p),
                 ("blank_label", C.c_int), ("maxT", C.c_int), ("maxU", C.c_int),
                 ("batch_first", C.c_bool)]
+
+
+class rnntGradOptions(C.Structure):
+    """include/rnnt.h `struct rnntGradOptions` (8 bytes, by value; zero = both options off)."""
+    _fields_ = [("fastemit_lambda", C.c_float), ("clamp", C.c_float)]
 
 
 RNNT_CPU, RNNT_GPU = 0, 1
@@ -62,6 +68,13 @@ _lib.rnnt_b200_loss_async_layout.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_in
 _lib.rnnt_b200_loss_async_layout_fp64.restype = C.c_int
 _lib.rnnt_b200_loss_async_layout_fp64.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double, _P, rnntOptions]
 RNNT_B200_LAYOUT_NTUV, RNNT_B200_LAYOUT_TUNV = 0, 1
+RNNT_B200_FP32, RNNT_B200_FP64 = 0, 3
+_lib.rnnt_b200_loss_async_ex.restype = C.c_int
+_lib.rnnt_b200_loss_async_ex.argtypes = [C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
+                                         rnntGradOptions, _P, rnntOptions]
+_lib.rnnt_b200_backward_ex.restype = C.c_int
+_lib.rnnt_b200_backward_ex.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
+                                       rnntGradOptions, _P, rnntOptions]
 _lib.get_workspace_size.restype = C.c_int
 _lib.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
 _lib.get_warprnnt_version.restype = C.c_int
@@ -175,11 +188,39 @@ def gpu_rnnt(acts, labels, input_lengths, label_lengths, costs, grads, blank_lab
     return 0
 
 
+_FLOAT32_MAX = 3.4028234663852886e38
+
+
+def grad_options(fastemit_lambda=0.0, clamp=-1.0):
+    """Checked rnntGradOptions for the *_ex entries, or None when both options are off (the plain entries
+    then run).  fastemit_lambda: finite, >= 0 (0 = off).  clamp: > 0 clips each gradient element to
+    [-clamp, clamp] before grad_scale and the upstream gradient are applied; <= 0 = off; not NaN."""
+    lam, c = float(fastemit_lambda), float(clamp)
+    if not (math.isfinite(lam) and 0.0 <= lam <= _FLOAT32_MAX):
+        raise ValueError("fastemit_lambda must be finite and >= 0 (float32), got %r" % (fastemit_lambda,))
+    if math.isnan(c):
+        raise ValueError("clamp must not be NaN")
+    if lam == 0.0 and not c > 0.0:
+        return None
+    return rnntGradOptions(lam, c)
+
+
+def _dtype_code(acts):
+    code = {torch.float32: RNNT_B200_FP32, torch.float64: RNNT_B200_FP64, torch.bfloat16: RNNT_B200_BF16,
+            torch.float16: RNNT_B200_FP16}.get(acts.dtype)
+    if code is None:
+        raise TypeError("unsupported data type %s" % acts.dtype)
+    return code
+
+
 def gpu_rnnt_async(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                   grad_scale=1.0, workspace=None):
+                   grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0):
     """Extension: no host synchronisation, `costs` on the device, gradients pre-multiplied by
-    `grad_scale`.  Returns the workspace tensor (keep it alive until the stream has run)."""
+    `grad_scale`.  Returns the workspace tensor (keep it alive until the stream has run).
+    fastemit_lambda / clamp: gradient options (see grad_options); the costs do not depend on them, and
+    with FastEmit on the gradient is not the gradient of the costs."""
     N, T, U, V = acts.shape
+    gopt = grad_options(fastemit_lambda, clamp)
     code = _code16(acts)
     if code:
         esz = 4
@@ -196,18 +237,23 @@ def gpu_rnnt_async(acts, labels, input_lengths, label_lengths, costs, grads, bla
         args = (acts.data_ptr(), _ptr(grads), _labels_ptr(labels), label_lengths.data_ptr(),
                 input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale, workspace.data_ptr(),
                 _options(acts, blank_label))
-        st = _lib.rnnt_b200_loss_async_16(code, *args) if code else fn(*args)
+        if gopt is not None:
+            st = _lib.rnnt_b200_loss_async_ex(_dtype_code(acts), RNNT_B200_LAYOUT_NTUV, *args[:-2], gopt, *args[-2:])
+        else:
+            st = _lib.rnnt_b200_loss_async_16(code, *args) if code else fn(*args)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("compute_rnnt_loss_async failed: " + status_string(st))
     return workspace
 
 
 def gpu_rnnt_async_tunv(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                        grad_scale=1.0, workspace=None):
+                        grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0):
     """Time-major extension: `acts` / `grads` are [T, U, N, V] (the layout the reference's CPU path
     indexes for batch_first == false, cpu_rnnt.h:139-144); labels [N, U-1], lengths and costs [N].
-    fp32 / fp64, no host synchronisation.  Returns the workspace tensor."""
+    fp32 / fp64, no host synchronisation.  Returns the workspace tensor.  Gradient options as
+    gpu_rnnt_async."""
     T, U, N, V = acts.shape
+    gopt = grad_options(fastemit_lambda, clamp)
     fn, esz = _pick(acts, "rnnt_b200_loss_async_layout", "rnnt_b200_loss_async_layout_fp64")
     with torch.cuda.device(acts.device):
         need = workspace_size(T, U, N, esz)
@@ -215,9 +261,13 @@ def gpu_rnnt_async_tunv(acts, labels, input_lengths, label_lengths, costs, grads
             workspace = torch.empty(need, dtype=torch.uint8, device=acts.device)
         opt = _options(acts, blank_label)
         opt.maxT, opt.maxU = T, U
-        st = fn(RNNT_B200_LAYOUT_TUNV, acts.data_ptr(), _ptr(grads), _labels_ptr(labels),
-                label_lengths.data_ptr(), input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale,
-                workspace.data_ptr(), opt)
+        args = (acts.data_ptr(), _ptr(grads), _labels_ptr(labels), label_lengths.data_ptr(),
+                input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale)
+        if gopt is not None:
+            st = _lib.rnnt_b200_loss_async_ex(_dtype_code(acts), RNNT_B200_LAYOUT_TUNV, *args, gopt,
+                                              workspace.data_ptr(), opt)
+        else:
+            st = fn(RNNT_B200_LAYOUT_TUNV, *args, workspace.data_ptr(), opt)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_loss_async_layout failed: " + status_string(st))
     return workspace
@@ -261,17 +311,23 @@ def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_la
 
 
 def gpu_rnnt_backward(acts, labels, input_lengths, label_lengths, grads, grad_costs, blank_label,
-                      grad_scale, workspace):
+                      grad_scale, workspace, *, fastemit_lambda=0.0, clamp=-1.0):
     """Second half: grads[b] = grad_scale * grad_costs[b] * d cost[b] / d acts[b] from the lattices
-    gpu_rnnt_forward left in `workspace` (grad_costs: device tensor [N] or None for ones)."""
+    gpu_rnnt_forward left in `workspace` (grad_costs: device tensor [N] or None for ones).
+    With gradient options (see grad_options): grad_scale * grad_costs[b] * clip(g[b]), g[b] the FastEmit
+    gradient when fastemit_lambda > 0."""
     N, T, U, V = acts.shape
+    gopt = grad_options(fastemit_lambda, clamp)
     code = _code16(acts)
     fn = None if code else _pick(acts, "rnnt_b200_backward", "rnnt_b200_backward_fp64")[0]
     with torch.cuda.device(acts.device):
         args = (acts.data_ptr(), grads.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(),
                 input_lengths.data_ptr(), V, N, _ptr(grad_costs), grad_scale, workspace.data_ptr(),
                 _options(acts, blank_label))
-        st = _lib.rnnt_b200_backward_16(code, *args) if code else fn(*args)
+        if gopt is not None:
+            st = _lib.rnnt_b200_backward_ex(_dtype_code(acts), *args[:-2], gopt, *args[-2:])
+        else:
+            st = _lib.rnnt_b200_backward_16(code, *args) if code else fn(*args)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_backward failed: " + status_string(st))
     return 0
