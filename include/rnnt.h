@@ -331,7 +331,10 @@ int rnnt_b200_profile_collect(float* ms3_mean);
  *      for the chunk kernels);  1  1 if those lanes are `32 / lanes` apart in the warp (bank-aware mapping), 0 if adjacent;
  *   2  label columns per lane of the fp32 wavefront for maxU = a;  3  its threads per utterance and direction;
  *   4  diagonals of its factor ring (b != 0: next to the streaming passes of other batch groups);
- *   5  split-K slabs of the additive joint's S product for alphabet size a.   Returns -1 for an unknown `what`. */
+ *   5  split-K slabs of the additive joint's S product for alphabet size a;
+ *   6  as 1, but with the RNNT_B200_CHUNK_MAP tuning hook applied (the mapping the chunk kernels are given);
+ *   7  1 if the RNNT_B200_PDL tuning hook asks for programmatic dependent launch, else 0.
+ * 4, 5 and 6 honour the tuning hooks (README), 0 and 1 do not.   Returns -1 for an unknown `what`. */
 int rnnt_b200_debug_policy(int what, int a, int b);
 
 /* Build identification string, e.g. "b200-rnnt sm_90a <date>". */

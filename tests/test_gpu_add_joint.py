@@ -5,15 +5,9 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import pyoracle
+from joint_reference import assert_joint_close, grad_mismatch, reference
 
 pytestmark = pytest.mark.gpu
-
-
-def reference(trans, pred, labels, tl, ul, blank):
-    acts = trans[:, :, None, :].astype(np.float64) + pred[:, None, :, :].astype(np.float64)
-    c, g, _ = pyoracle.rnnt_logits(acts, labels, tl, ul, blank)
-    return c, g.sum(axis=2), g.sum(axis=1)
 
 
 @pytest.mark.parametrize("shape", [(3, 9, 5, 28, 0), (2, 17, 34, 13, 4), (4, 30, 8, 300, 0),
@@ -43,10 +37,8 @@ def test_add_joint_matches_dense_oracle(shape):
                                                           torch.as_tensor(ul).cuda())
     w = torch.linspace(0.5, 1.5, N, device="cuda")
     (out * w).sum().backward()
-    wn = w.cpu().numpy()[:, None, None]
-    assert np.allclose(out.detach().cpu().numpy(), c_ref, rtol=1e-5, atol=1e-5)
-    assert np.allclose(tt.grad.cpu().numpy(), df_ref * wn, rtol=1e-4, atol=2e-6)
-    assert np.allclose(pp.grad.cpu().numpy(), dg_ref * wn, rtol=1e-4, atol=2e-6)
+    assert_joint_close(out.detach().cpu().numpy(), tt.grad.cpu().numpy(), pp.grad.cpu().numpy(), c_ref, df_ref, dg_ref,
+                       labels, tl, ul, blank, scale=w.cpu().numpy())
 
 
 def test_add_joint_equals_dense_operator_and_reductions():
@@ -69,8 +61,10 @@ def test_add_joint_equals_dense_operator_and_reductions():
         dense = RNNTLoss(reduction=reduction)(acts.contiguous(), labels, tl, ul)
         dense.backward()
         assert torch.allclose(loss, dense, rtol=1e-5)
-        assert torch.allclose(g1, trans.grad, rtol=1e-4, atol=2e-6)
-        assert torch.allclose(g2, pred.grad, rtol=1e-4, atol=2e-6)
+        lab_np, tl_np, ul_np = labels.cpu().numpy(), tl.cpu().numpy(), ul.cpu().numpy()
+        problems = grad_mismatch(g1.cpu().numpy(), trans.grad.double().cpu().numpy(), tl_np, lab_np, ul_np, 0, "dF") + \
+            grad_mismatch(g2.cpu().numpy(), pred.grad.double().cpu().numpy(), ul_np + 1, lab_np, ul_np, 0, "dG")
+        assert not problems, "\n".join(problems)
     with pytest.raises(ValueError):
         add_joint_rnnt_loss(trans, pred[:, :-1].contiguous(), labels, tl, ul)
     with pytest.raises(RuntimeError):

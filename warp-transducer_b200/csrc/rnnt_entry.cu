@@ -393,6 +393,12 @@ inline bool chunk_enabled() {
     static const bool on = [] { const char* e = getenv("RNNT_B200_CHUNK"); return !(e && atoi(e) == 0); }();
     return on;
 }
+// lane mapping of the chunk kernels: bank-aware choice, or what RNNT_B200_CHUNK_MAP = 0 | 1 forces (tuning hook)
+inline int chunk_hmajor(int V, int tpr, int elt) {
+    static const int forced_map = [] { const char* e = getenv("RNNT_B200_CHUNK_MAP"); return e ? atoi(e) : -1; }();
+    if (forced_map == 0 || forced_map == 1) return forced_map;
+    return chunk_walk_cost(V, tpr, elt, true) < chunk_walk_cost(V, tpr, elt, false);
+}
 template <typename T>
 bool chunk_pass(const T* acts, T* grads, const int* labels, const int* xlen, const int* ylen,
                 const Workspace& w, T scale, const T* scale_vec, const Dims& d, cudaStream_t s, int pass,
@@ -415,13 +421,15 @@ bool chunk_pass(const T* acts, T* grads, const int* labels, const int* xlen, con
     const size_t smem = (size_t)rows_per * d.V * sizeof(T);
     const bool scaled = scale != T(1) || scale_vec;
     static const uint32_t wait_ns = [] { const char* e = getenv("RNNT_B200_CHUNK_WAIT_NS"); return e ? (uint32_t)atoi(e) : 2000u; }();
-    static const int forced_map = [] { const char* e = getenv("RNNT_B200_CHUNK_MAP"); return e ? atoi(e) : -1; }();
-    int hmajor = chunk_walk_cost(d.V, tpr, (int)sizeof(T), true) < chunk_walk_cost(d.V, tpr, (int)sizeof(T), false);
-    if (forced_map == 0 || forced_map == 1) hmajor = forced_map;   // tuning hook
-    // 8+ chunk CTAs per SM need most of the shared memory: ask for the largest carve-out once per kernel
-    auto prefer_smem = [](auto kernel) {
+    const int hmajor = chunk_hmajor(d.V, tpr, (int)sizeof(T));
+    // 8+ chunk CTAs per SM need most of the shared memory: ask for the largest carve-out once per kernel.
+    // The chosen lane count keeps a chunk at <= 32 KB; a forced smaller one (CHUNK_TPR) stages more rows of the
+    // same length, up to 128 KB (fp32, V = 128, one lane per row), which a launch gets only after opting in.
+    auto prefer_smem = [smem](auto kernel) {
         func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributePreferredSharedMemoryCarveout,
                        cudaSharedmemCarveoutMaxShared);
+        if (smem > 32 * 1024)
+            func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         return kernel;
     };
     auto go = [&](auto tpr_c, auto nt_c) {
@@ -480,6 +488,12 @@ void stream_pass(const IO* acts, IO* grads, const int* labels, const int* xlen, 
         stream_passes<T, (sizeof(IO) == 4 ? 2 : 1), IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass, ro);
     else
         stream_passes<T, 1, IO>(acts, grads, labels, xlen, ylen, w, scale, scale_vec, d, s, pass, ro);
+}
+
+// RNNT_B200_PDL=1 (tuning hook, experimental): programmatic dependent launch, see run()
+inline bool pdl_requested() {
+    static const bool on = [] { const char* e = getenv("RNNT_B200_PDL"); return e && atoi(e) != 0; }();
+    return on;
 }
 
 // What a call does.  The reference API is FULL (stats -> lattice -> grad in one call); the
@@ -657,8 +671,7 @@ rnntStatus_t run(const IO* acts, IO* grads, const int* labels, const int* ylen, 
     // the tail of the kernel before them; each waits (griddepcontrol.wait) before it touches that kernel's
     // output.  The three kernels are each bound by their own latency chains rather than by the launch gaps,
     // so it stays opt-in.  (The event markers of the profiling mode would serialise the kernels anyway.)
-    static const bool pdl_env = [] { const char* e = getenv("RNNT_B200_PDL"); return e && atoi(e) != 0; }();
-    g_pdl = pdl_env && groups == 1 && !g_profile;
+    g_pdl = pdl_requested() && groups == 1 && !g_profile;
     if (groups == 1) {
         const Group g = make_group(0, N);
         if (phase != kBackward) {
@@ -1316,6 +1329,8 @@ int rnnt_b200_debug_policy(int what, int a, int b) {
         case 3: return lattice_threads(a);
         case 4: return lattice_ring_depth(a, b != 0);
         case 5: return joint_slices(a);
+        case 6: return (size_t)a * (size_t)b > 512 || a <= 0 ? 0 : chunk_hmajor(a, pick_tpr(a), b);
+        case 7: return pdl_requested() ? 1 : 0;
         default: return -1;
     }
 }
