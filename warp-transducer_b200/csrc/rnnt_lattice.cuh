@@ -383,10 +383,9 @@ inline int lattice_threads(int maxU) {
 // Diagonals of factors each thread keeps in flight.  8 covers the DRAM latency of an otherwise idle GPU
 // (8 steps x ~220 ns); next to the streaming passes of other batch groups the loaded latency is several
 // microseconds and the multi-warp wavefront starves, so there the ring is as deep as ~100 KB allow.
-// RNNT_B200_LAT_RING = 8 | 16 | 32 forces it (tuning hook).
-inline int lattice_ring_depth(int maxU, bool co_running) {
+// forced = 8 | 16 | 32 (tuning hook RNNT_B200_LAT_RING) overrides it where the ring fits.
+inline int lattice_ring_depth(int maxU, bool co_running, int forced) {
     if (maxU <= 64) return 8;
-    static const int forced = [] { const char* e = getenv("RNNT_B200_LAT_RING"); return e ? atoi(e) : 0; }();
     const size_t per_slot = (size_t)lattice_threads(maxU) * lattice_cols(maxU) * 16;
     int depth = 8;
     if (co_running)

@@ -213,6 +213,38 @@ def _dtype_code(acts):
     return code
 
 
+def _ex_options(fastemit_lambda, clamp):
+    """rnntGradOptions for the *_ex entries; zeroed (both off) they launch exactly the plain entries' kernels."""
+    gopt = grad_options(fastemit_lambda, clamp)
+    return rnntGradOptions() if gopt is None else gopt
+
+
+def _workspace(acts, T, U, N, workspace):
+    """`workspace` when it holds the bytes these extents need, else a new one on the activations' device."""
+    need = workspace_size(T, U, N, 8 if acts.dtype == torch.float64 else 4)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=acts.device)
+    return workspace
+
+
+def _loss_async(layout, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
+                grad_scale, workspace, fastemit_lambda, clamp):
+    gopt = _ex_options(fastemit_lambda, clamp)
+    code = _dtype_code(acts)
+    if layout == RNNT_B200_LAYOUT_TUNV and code not in (RNNT_B200_FP32, RNNT_B200_FP64):
+        raise TypeError("unsupported data type %s for the time-major layout" % acts.dtype)
+    with torch.cuda.device(acts.device):
+        workspace = _workspace(acts, T, U, N, workspace)
+        opt = _options(acts, blank_label)
+        opt.maxT, opt.maxU = T, U
+        st = _lib.rnnt_b200_loss_async_ex(code, layout, acts.data_ptr(), _ptr(grads), _labels_ptr(labels),
+                                          label_lengths.data_ptr(), input_lengths.data_ptr(), V, N,
+                                          costs.data_ptr(), grad_scale, gopt, workspace.data_ptr(), opt)
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_loss_async_ex failed: " + status_string(st))
+    return workspace
+
+
 def gpu_rnnt_async(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
                    grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0):
     """Extension: no host synchronisation, `costs` on the device, gradients pre-multiplied by
@@ -220,30 +252,8 @@ def gpu_rnnt_async(acts, labels, input_lengths, label_lengths, costs, grads, bla
     fastemit_lambda / clamp: gradient options (see grad_options); the costs do not depend on them, and
     with FastEmit on the gradient is not the gradient of the costs."""
     N, T, U, V = acts.shape
-    gopt = grad_options(fastemit_lambda, clamp)
-    code = _code16(acts)
-    if code:
-        esz = 4
-    elif acts.dtype == torch.float32:
-        fn, esz = _lib.compute_rnnt_loss_async, 4
-    elif acts.dtype == torch.float64:
-        fn, esz = _lib.compute_rnnt_loss_async_fp64, 8
-    else:
-        raise TypeError("unsupported data type %s" % acts.dtype)
-    with torch.cuda.device(acts.device):
-        need = workspace_size(T, U, N, esz)
-        if workspace is None or workspace.numel() < need:
-            workspace = torch.empty(need, dtype=torch.uint8, device=acts.device)
-        args = (acts.data_ptr(), _ptr(grads), _labels_ptr(labels), label_lengths.data_ptr(),
-                input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale, workspace.data_ptr(),
-                _options(acts, blank_label))
-        if gopt is not None:
-            st = _lib.rnnt_b200_loss_async_ex(_dtype_code(acts), RNNT_B200_LAYOUT_NTUV, *args[:-2], gopt, *args[-2:])
-        else:
-            st = _lib.rnnt_b200_loss_async_16(code, *args) if code else fn(*args)
-    if st != RNNT_STATUS_SUCCESS:
-        raise RuntimeError("compute_rnnt_loss_async failed: " + status_string(st))
-    return workspace
+    return _loss_async(RNNT_B200_LAYOUT_NTUV, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads,
+                       blank_label, grad_scale, workspace, fastemit_lambda, clamp)
 
 
 def gpu_rnnt_async_tunv(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
@@ -253,24 +263,8 @@ def gpu_rnnt_async_tunv(acts, labels, input_lengths, label_lengths, costs, grads
     fp32 / fp64, no host synchronisation.  Returns the workspace tensor.  Gradient options as
     gpu_rnnt_async."""
     T, U, N, V = acts.shape
-    gopt = grad_options(fastemit_lambda, clamp)
-    fn, esz = _pick(acts, "rnnt_b200_loss_async_layout", "rnnt_b200_loss_async_layout_fp64")
-    with torch.cuda.device(acts.device):
-        need = workspace_size(T, U, N, esz)
-        if workspace is None or workspace.numel() < need:
-            workspace = torch.empty(need, dtype=torch.uint8, device=acts.device)
-        opt = _options(acts, blank_label)
-        opt.maxT, opt.maxU = T, U
-        args = (acts.data_ptr(), _ptr(grads), _labels_ptr(labels), label_lengths.data_ptr(),
-                input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale)
-        if gopt is not None:
-            st = _lib.rnnt_b200_loss_async_ex(_dtype_code(acts), RNNT_B200_LAYOUT_TUNV, *args, gopt,
-                                              workspace.data_ptr(), opt)
-        else:
-            st = fn(RNNT_B200_LAYOUT_TUNV, *args, workspace.data_ptr(), opt)
-    if st != RNNT_STATUS_SUCCESS:
-        raise RuntimeError("rnnt_b200_loss_async_layout failed: " + status_string(st))
-    return workspace
+    return _loss_async(RNNT_B200_LAYOUT_TUNV, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads,
+                       blank_label, grad_scale, workspace, fastemit_lambda, clamp)
 
 
 def _code16(acts):
@@ -282,25 +276,17 @@ def costs_dtype(acts):
     return torch.float32 if _code16(acts) else acts.dtype
 
 
-def _pick(acts, f32, f64):
-    if acts.dtype == torch.float32:
-        return getattr(_lib, f32), 4
-    if acts.dtype == torch.float64:
-        return getattr(_lib, f64), 8
-    raise TypeError("unsupported data type %s" % acts.dtype)
-
-
 def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_label,
                      prepare_backward=True, workspace=None):
     """Training-step split, first half: statistics + lattices into `workspace`, costs on the
     device, no synchronisation.  Returns the workspace tensor (hand it to gpu_rnnt_backward)."""
     N, T, U, V = acts.shape
     code = _code16(acts)
-    fn, esz = (None, 4) if code else _pick(acts, "rnnt_b200_forward", "rnnt_b200_forward_fp64")
+    fn = {torch.float32: _lib.rnnt_b200_forward, torch.float64: _lib.rnnt_b200_forward_fp64}.get(acts.dtype)
+    if code is None and fn is None:
+        raise TypeError("unsupported data type %s" % acts.dtype)
     with torch.cuda.device(acts.device):
-        need = workspace_size(T, U, N, esz)
-        if workspace is None or workspace.numel() < need:
-            workspace = torch.empty(need, dtype=torch.uint8, device=acts.device)
+        workspace = _workspace(acts, T, U, N, workspace)
         args = (acts.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(), input_lengths.data_ptr(),
                 V, N, costs.data_ptr(), 1 if prepare_backward else 0, workspace.data_ptr(),
                 _options(acts, blank_label))
@@ -317,19 +303,14 @@ def gpu_rnnt_backward(acts, labels, input_lengths, label_lengths, grads, grad_co
     With gradient options (see grad_options): grad_scale * grad_costs[b] * clip(g[b]), g[b] the FastEmit
     gradient when fastemit_lambda > 0."""
     N, T, U, V = acts.shape
-    gopt = grad_options(fastemit_lambda, clamp)
-    code = _code16(acts)
-    fn = None if code else _pick(acts, "rnnt_b200_backward", "rnnt_b200_backward_fp64")[0]
+    gopt = _ex_options(fastemit_lambda, clamp)
+    code = _dtype_code(acts)
     with torch.cuda.device(acts.device):
-        args = (acts.data_ptr(), grads.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(),
-                input_lengths.data_ptr(), V, N, _ptr(grad_costs), grad_scale, workspace.data_ptr(),
-                _options(acts, blank_label))
-        if gopt is not None:
-            st = _lib.rnnt_b200_backward_ex(_dtype_code(acts), *args[:-2], gopt, *args[-2:])
-        else:
-            st = _lib.rnnt_b200_backward_16(code, *args) if code else fn(*args)
+        st = _lib.rnnt_b200_backward_ex(code, acts.data_ptr(), grads.data_ptr(), _labels_ptr(labels),
+                                        label_lengths.data_ptr(), input_lengths.data_ptr(), V, N, _ptr(grad_costs),
+                                        grad_scale, gopt, workspace.data_ptr(), _options(acts, blank_label))
     if st != RNNT_STATUS_SUCCESS:
-        raise RuntimeError("rnnt_b200_backward failed: " + status_string(st))
+        raise RuntimeError("rnnt_b200_backward_ex failed: " + status_string(st))
     return 0
 
 
