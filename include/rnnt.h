@@ -306,6 +306,63 @@ rnntStatus_t rnnt_b200_add_joint_backward_ex(const float* trans, const float* pr
                                              float grad_scale, struct rnntGradOptions grad_options,
                                              void* workspace, struct rnntOptions options);
 
+/*
+ * Pruned RNN-T loss (Kuang et al., "Pruned RNN-T for fast, memory-efficient ASR training", Interspeech 2022).
+ * activations [minibatch, maxT, s_range, alphabet_size]: row (b, t, s) holds the logits of lattice cell
+ * (t, u = ranges[b*maxT + t] + s); ranges [minibatch, maxT] int32 window starts (any values); labels, lengths and
+ * costs as rnnt_b200_loss_async_ex; options.maxU is the full lattice width (max label length + 1).
+ * The loss is the RNN-T loss over the paths that only visit cells covered by a row of their frame, on the dense
+ * [T_b, U_b] lattice: a cell with no row has log-zero blank and label factors, a covered cell takes its blank logit
+ * and, for u < U_b - 1, the logit of y_u from its own row.  A row with t >= T_b, u < 0 or u >= U_b is padding: not
+ * read by the forward, zero gradient.  The gradient of a valid row is the dense formula at (b, t, u).  An utterance
+ * with no surviving path costs +inf and gets an all-zero gradient.  With s_range = maxU and ranges == 0 this is
+ * exactly rnnt_b200_loss_async_ex, bitwise.
+ * dtype: RNNT_B200_FP32 / _FP64 / _BF16 / _FP16 (costs double* for fp64, float* otherwise); layout must be
+ * RNNT_B200_LAYOUT_NTUV; s_range >= 1; minibatch * maxT * s_range < 2^31; ranges a DEVICE pointer.  The gradient
+ * options are those of rnnt_b200_loss_async_ex.  Workspace from rnnt_b200_pruned_workspace_size.
+ */
+rnntStatus_t rnnt_b200_pruned_workspace_size(int maxT, int maxU, int s_range, int minibatch, size_t dtype_size,
+                                             size_t* size_bytes);
+rnntStatus_t rnnt_b200_pruned_loss_async_ex(int dtype, int layout, const void* activations, void* gradients,
+                                            const int* ranges, int s_range, const int* flat_labels,
+                                            const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                            int minibatch, void* costs_device, double grad_scale,
+                                            struct rnntGradOptions grad_options, void* workspace,
+                                            struct rnntOptions options);
+/* Training-step split of the same (rnnt_b200_forward / rnnt_b200_backward_ex); the backward half reads the
+ * lattices the forward left in `workspace` and must get the same ranges. */
+rnntStatus_t rnnt_b200_pruned_forward(int dtype, const void* activations, const int* ranges, int s_range,
+                                      const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                      int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
+                                      void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_backward_ex(int dtype, const void* activations, void* gradients, const int* ranges,
+                                          int s_range, const int* flat_labels, const int* label_lengths,
+                                          const int* input_lengths, int alphabet_size, int minibatch,
+                                          const void* grad_costs_device, double grad_scale,
+                                          struct rnntGradOptions grad_options, void* workspace,
+                                          struct rnntOptions options);
+
+/*
+ * Pruning ranges from the additive joint's lattice: call after rnnt_b200_add_joint_forward with
+ * prepare_backward = 1 (or a full rnnt_b200_add_joint_loss with gradients) on the same workspace, stream and
+ * options.  Writes ranges [minibatch, options.maxT] (DEVICE int32).  Per utterance, with R = s_range >= 2 and
+ * E = max(U_b - R, 0), for cell (t,u)
+ *   e_b(t,u) = exp(alpha(t,u) + lp_blank(t,u) + beta(t+1,u) - ll)      (blank occupancy)
+ *   e_y(t,u) = exp(alpha(t,u) + lp_y(t,u) + beta(t,u+1) - ll)          (label occupancy)
+ *   1. For 0 < t < T_b - 1, s[t] is the smallest a in [0, E] maximising
+ *      sum_{u=a}^{min(a+R,U_b)-1} e_b(t,u) - [a>0] e_y(t,a-1).  This is k2's criterion.
+ *   2. Set s[0] = 0.  If T_b > 1, set s[T_b-1] = E.  For t >= T_b, set s[t] = E.
+ *   3. Sweep once, for t = T_b-2 down to 0: s[t] = min(max(s[t], s[t+1] - (R-1)), s[t+1]).
+ * After the sweep the windows are non-decreasing, consecutive windows overlap (no label is skipped), the last frame
+ * covers U_b - 1 when T_b > 1, and, for T_b > 1, s[0] == 0 leaves a path while an utterance without one
+ * (E > (T_b-1)(R-1)) ends with s[0] > 0.  A path can still be lost when frame 1's best window starts beyond R - 1
+ * (DESIGN.md §8); the pruned loss then reports +inf for that utterance.
+ * Returns RNNT_STATUS_INVALID_VALUE for s_range < 2, NULL pointers, or extents the joint does not accept.
+ */
+rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const int* input_lengths, int minibatch,
+                                              int s_range, int* ranges, const void* workspace,
+                                              struct rnntOptions options);
+
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug
  * builds (include/detail/cpu_rnnt.h:167-170); tests/test_gpu_round2.py does the same.  Synchronises. */

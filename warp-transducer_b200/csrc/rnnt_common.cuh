@@ -16,7 +16,7 @@ constexpr int kWarp = 32;
 // ---------------------------------------------------------------------------------------------
 struct FastDiv {
     uint32_t d, mul, shr;
-    FastDiv() : d(1), mul(0), shr(0) {}
+    __host__ __device__ FastDiv() : d(1), mul(0), shr(0) {}
     explicit FastDiv(uint32_t div) : d(div) {
         if (div <= 1) {
             mul = 0;

@@ -292,6 +292,7 @@ struct Call {
     double scale;            // gradient multiplier, rounded to the arithmetic type
     const void* scale_vec;   // per-utterance gradient multipliers in the arithmetic type, or NULL
     rnntGradOptions grad;
+    bool pruned = false;     // logits [N,maxT,R,V] over the windows Tensors::ranges (DESIGN.md §8)
 };
 Call full_call(double scale, bool async = true, bool tunv = false, rnntGradOptions grad = {0.0f, 0.0f}) {
     return Call{kFull, async, false, tunv, scale, nullptr, grad};
@@ -313,6 +314,8 @@ struct Tensors {
     void* costs;   // arithmetic type; NULL in the backward phase
     void* workspace;
     rnntOptions opt;
+    const int* ranges = nullptr;   // pruned calls: [N, maxT] window starts
+    int s_range = 0;               // pruned calls: R, rows per frame
 };
 
 // The checks of every compute call, all before any device access; the first that fails decides the status.
@@ -322,6 +325,9 @@ rnntStatus_t check_call(const Tensors& t, const Call& c) {
     if (!t.acts || !t.labels || !t.ylen || !t.xlen || (!t.costs && c.phase != kBackward) || !t.workspace ||
         t.V <= 0 || t.N <= 0 || opt.maxT <= 0 || opt.maxU <= 0 || (c.phase == kBackward && !t.grads))
         return RNNT_STATUS_INVALID_VALUE;  // reference src/rnnt_entrypoint.cpp:49-59
+    // pruned rows are counted with 32 bits like the dense ones; the pruned kernels index [N,maxT,R,V] only
+    if (c.pruned && (!t.ranges || t.s_range < 1 || c.tunv || (uint64_t)t.N * opt.maxT * t.s_range >= (1ull << 31)))
+        return RNNT_STATUS_INVALID_VALUE;
     if (opt.loc == RNNT_CPU) {
         fprintf(stderr, "b200-rnnt: CPU execution requested, but this library is the CUDA path only\n");
         return RNNT_STATUS_EXECUTION_FAILED;
@@ -367,6 +373,8 @@ struct Group {
     GradReg<T> gr;
     cudaStream_t s;      // the call's stream (the grouped schedule runs each lattice on a side stream)
     bool pdl;            // launch the dependent kernels with programmatic stream serialization
+    bool pruned;         // the *_pruned_kernel instantiations, given `pr`
+    Prune pr;
     bool scaled() const { return scale != T(1) || scale_vec; }
 };
 
@@ -377,7 +385,21 @@ struct Group {
 template <typename T, int VEC, int NV, typename IO>
 void launch_row(const Group<T, IO>& g, int pass) {
     using Val = const typename Lat<T>::val*;
-    if (pass == 1) {
+    if (g.pruned) {
+        if (pass == 1) {
+            rowstats_row_pruned_kernel<T, VEC, NV, IO><<<g.d.rows, RowThreads<IO>::value, 0, g.s>>>(
+                g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
+                static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d, g.pr);
+        } else {
+            auto k = g.reg ? (g.scaled() ? grad_row_pruned_kernel<T, VEC, NV, true, IO, true>
+                                         : grad_row_pruned_kernel<T, VEC, NV, false, IO, true>)
+                           : (g.scaled() ? grad_row_pruned_kernel<T, VEC, NV, true, IO, false>
+                                         : grad_row_pruned_kernel<T, VEC, NV, false, IO, false>);
+            launch_k(k, dim3(g.d.rows), dim3(RowThreads<IO>::value), 0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen,
+                     g.ylen, static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
+                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
+        }
+    } else if (pass == 1) {
         rowstats_row_kernel<T, VEC, NV, IO><<<g.d.rows, RowThreads<IO>::value, 0, g.s>>>(
             g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
             static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d);
@@ -398,7 +420,21 @@ void launch_tile(const Group<T, IO>& g, int pass) {
     using Val = const typename Lat<T>::val*;
     const uint64_t warps = ((uint64_t)g.d.rows * LPR + 31) / 32;
     const unsigned grid = (unsigned)((warps + 7) / 8);
-    if (pass == 1) {
+    if (g.pruned) {
+        if (pass == 1) {
+            rowstats_tile_pruned_kernel<T, VEC, LPR, IO><<<grid, 256, 0, g.s>>>(
+                g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
+                static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d, g.pr);
+        } else {
+            auto k = g.reg ? (g.scaled() ? grad_tile_pruned_kernel<T, VEC, LPR, true, IO, true>
+                                         : grad_tile_pruned_kernel<T, VEC, LPR, false, IO, true>)
+                           : (g.scaled() ? grad_tile_pruned_kernel<T, VEC, LPR, true, IO, false>
+                                         : grad_tile_pruned_kernel<T, VEC, LPR, false, IO, false>);
+            launch_k(k, dim3(grid), dim3(256), 0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen,
+                     static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
+                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
+        }
+    } else if (pass == 1) {
         rowstats_tile_kernel<T, VEC, LPR, IO><<<grid, 256, 0, g.s>>>(
             g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
             static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d);
@@ -523,7 +559,22 @@ bool chunk_pass(const Group<T, T>& g, int pass) {
     auto go = [&](auto tpr_c, auto nt_c) {
         constexpr int TPR = decltype(tpr_c)::value, NT = decltype(nt_c)::value;
         if constexpr (NT / TPR >= 4) {
-            if (pass == 1)
+            if (g.pruned) {
+                if (pass == 1) {
+                    prefer_smem(rowstats_chunk_pruned_kernel<T, TPR, NT>)<<<grid, NT, smem, g.s>>>(
+                        g.acts, g.labels, g.xlen, g.ylen, static_cast<Pair*>(g.w.stat), static_cast<Fac*>(g.w.lp2), g.d,
+                        hmajor, wait_ns, g.pr);
+                } else {
+                    auto k = g.reg ? (g.scaled() ? grad_chunk_pruned_kernel<T, TPR, NT, true, true>
+                                                 : grad_chunk_pruned_kernel<T, TPR, NT, false, true>)
+                                   : (g.scaled() ? grad_chunk_pruned_kernel<T, TPR, NT, true, false>
+                                                 : grad_chunk_pruned_kernel<T, TPR, NT, false, false>);
+                    launch_k(prefer_smem(k), dim3(grid), dim3(NT), smem, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen,
+                             g.ylen, static_cast<const Pair*>(g.w.stat), static_cast<const Val*>(g.w.alphas),
+                             static_cast<const Val*>(g.w.betas), static_cast<const Val*>(g.w.llf), g.scale,
+                             g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr);
+                }
+            } else if (pass == 1)
                 prefer_smem(rowstats_chunk_kernel<T, TPR, NT>)<<<grid, NT, smem, g.s>>>(
                     g.acts, g.labels, g.xlen, g.ylen, static_cast<Pair*>(g.w.stat), static_cast<Fac*>(g.w.lp2), g.d,
                     hmajor, wait_ns);
@@ -610,7 +661,8 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
 
     g_last_launches = 0;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(opt.stream);
-    const uint64_t rows64 = (uint64_t)N * opt.maxT * opt.maxU;
+    const int rows_u = c.pruned ? t.s_range : opt.maxU;   // logit rows per frame (stat is carved per row)
+    const uint64_t rows64 = (uint64_t)N * opt.maxT * rows_u;
     const size_t lat = (size_t)N * (opt.maxT + opt.maxU - 1) * opt.maxU;
     Workspace w = carve(t.workspace, rows64, lat, N, opt.maxU, sizeof(T));
 
@@ -620,7 +672,8 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
     // rejecting it here would break every caller written against the reference.  The [T,U,N,V]
     // layout the reference's CPU path indexes (include/detail/cpu_rnnt.h:139-144) is available through
     // the explicit extension entry rnnt_b200_loss_async_layout (layout = RNNT_B200_LAYOUT_TUNV).
-    const Dims d = make_dims(t, c.tunv);
+    Dims d = make_dims(t, c.tunv);
+    d.rows = (uint32_t)rows64;
 
     // Integer inputs: device pointers are used in place; host pointers (the header's literal
     // contract, reference include/rnnt.h:84-89) are staged through the workspace.
@@ -664,8 +717,10 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
     // so it stays opt-in.  (The event markers of the profiling mode would serialise the kernels anyway.)
     const bool pdl = hooks().pdl && groups == 1 && !g_profile;
 
-    // ---- batch groups (Group).  One group = the plain in-order pipeline.
-    const size_t cell_stride = (size_t)opt.maxT * opt.maxU;            // rows per utterance
+    // ---- batch groups (Group).  One group = the plain in-order pipeline.  A pruned call's groups are offset by
+    // maxT * R logit rows per utterance, its lattices by maxT * maxU cells as a dense call's.
+    const size_t cell_stride = (size_t)opt.maxT * opt.maxU;            // lattice cells per utterance
+    const size_t row_stride = (size_t)opt.maxT * rows_u;               // logit rows per utterance
     const size_t lat_stride = (size_t)(opt.maxT + opt.maxU - 1) * opt.maxU;
     const size_t lab_stride = opt.maxU > 1 ? opt.maxU - 1 : 0;
     using Pair = typename Real<T>::pair;
@@ -674,7 +729,7 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
     auto make_group = [&](int b0, int nb) {
         Group<T, IO> g;
         g.w = w;
-        g.w.stat = static_cast<Pair*>(w.stat) + (size_t)b0 * cell_stride;
+        g.w.stat = static_cast<Pair*>(w.stat) + (size_t)b0 * row_stride;
         g.w.lp2 = static_cast<char*>(w.lp2) + (size_t)b0 * lat_stride * 16;
         // fp32 lattices are cell-major [b][t][u], fp64 ones diagonal-major (rnnt_kernels.cuh: cell / skew)
         const size_t val_stride = sizeof(T) == 4 ? cell_stride : lat_stride;
@@ -684,9 +739,9 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
         g.w.llb = static_cast<char*>(w.llb) + (size_t)b0 * 8;
         g.d = d;
         g.d.N = nb;
-        g.d.rows = (uint32_t)((size_t)nb * cell_stride);
-        g.acts = acts + (size_t)b0 * cell_stride * V;
-        g.grads = grads ? grads + (size_t)b0 * cell_stride * V : nullptr;
+        g.d.rows = (uint32_t)((size_t)nb * row_stride);
+        g.acts = acts + (size_t)b0 * row_stride * V;
+        g.grads = grads ? grads + (size_t)b0 * row_stride * V : nullptr;
         g.labels = labels + (size_t)b0 * lab_stride;
         g.xlen = xlen + b0;
         g.ylen = ylen + b0;
@@ -697,6 +752,8 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
         g.gr = make_grad_reg<T>(c.grad, g.w);
         g.s = s;
         g.pdl = pdl;
+        g.pruned = c.pruned;
+        g.pr = Prune{c.pruned ? t.ranges + (size_t)b0 * opt.maxT : nullptr, FastDiv((uint32_t)rows_u)};
         return g;
     };
     const bool with_beta = grads || c.want_beta;
@@ -729,6 +786,13 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
 
     profile_begin_call();
     mark(0, s);
+    if (c.pruned && c.phase != kBackward) {
+        // log-zero factors for the cells no row covers (pass 1 writes the covered ones): 16 B per lattice cell
+        using Fac = typename Lat<T>::fac;
+        lattice_fill_kernel<T><<<(unsigned)std::min<size_t>((lat + 255) / 256, 4096), 256, 0, s>>>(
+            static_cast<Fac*>(w.lp2), lat);
+        ++g_last_launches;
+    }
     if (groups == 1) {
         const Group<T, IO> g = make_group(0, N);
         if (c.phase != kBackward) {
@@ -814,6 +878,12 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
     JointWorkspace w;
     Carver c(base);
     const size_t C = (size_t)N * T * U, D = (size_t)N * (T + U - 1) * U;
+    // the lattice sections first: their offsets do not depend on V, so the pruning-ranges entry finds them
+    w.lp2 = c.take<float4>(D * 16);
+    w.alphas = c.take<LogVal>(D * 8);
+    w.betas = c.take<LogVal>(D * 8);
+    w.llf = c.take<LogVal>((size_t)N * 8);
+    w.llb = c.take<LogVal>((size_t)N * 8);
     w.ef = c.take<float>((size_t)N * T * V * 4);
     w.eg = c.take<float>((size_t)N * U * V * 4);
     w.mf = c.take<float>((size_t)N * T * 4);
@@ -823,11 +893,6 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
     w.bk = c.take<float>(C * 4);
     w.lb = c.take<float>(C * 4);
     w.part = c.take<float>(C * 4 * kJointSlices);
-    w.lp2 = c.take<float4>(D * 16);
-    w.alphas = c.take<LogVal>(D * 8);
-    w.betas = c.take<LogVal>(D * 8);
-    w.llf = c.take<LogVal>((size_t)N * 8);
-    w.llb = c.take<LogVal>((size_t)N * 8);
     w.bytes = c.off + 256;
     return w;
 }
@@ -1204,6 +1269,74 @@ rnntStatus_t rnnt_b200_add_joint_workspace_size(int maxT, int maxU, int minibatc
         return RNNT_STATUS_INVALID_VALUE;
     *size_bytes = carve_joint(nullptr, minibatch, maxT, maxU, alphabet_size).bytes;
     return RNNT_STATUS_SUCCESS;
+}
+
+// ---- pruned RNN-T loss (DESIGN.md §8): logits [N,maxT,R,V] over the windows `ranges` ---------------------
+rnntStatus_t rnnt_b200_pruned_workspace_size(int maxT, int maxU, int s_range, int minibatch, size_t dtype_size,
+                                             size_t* size_bytes) {
+    if (minibatch <= 0 || maxT <= 0 || maxU <= 0 || s_range < 1 || size_bytes == nullptr)
+        return RNNT_STATUS_INVALID_VALUE;
+    if (dtype_size != sizeof(double)) dtype_size = sizeof(float);
+    const size_t rows = (size_t)minibatch * maxT * s_range;
+    const size_t lat = (size_t)minibatch * (maxT + maxU - 1) * maxU;
+    *size_bytes = carve(nullptr, rows, lat, minibatch, maxU, dtype_size).bytes;
+    return RNNT_STATUS_SUCCESS;
+}
+
+rnntStatus_t rnnt_b200_pruned_loss_async_ex(int dtype, int layout, const void* activations, void* gradients,
+                                            const int* ranges, int s_range, const int* flat_labels,
+                                            const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                            int minibatch, void* costs_device, double grad_scale,
+                                            rnntGradOptions grad_options, void* workspace, rnntOptions options) {
+    if (!is_layout(layout)) return RNNT_STATUS_INVALID_VALUE;
+    Call c = full_call(grad_scale, true, layout == RNNT_B200_LAYOUT_TUNV, grad_options);
+    c.pruned = true;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options, ranges, s_range}, c);
+}
+
+rnntStatus_t rnnt_b200_pruned_forward(int dtype, const void* activations, const int* ranges, int s_range,
+                                      const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                      int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
+                                      void* workspace, rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.pruned = true;
+    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options, ranges, s_range}, c);
+}
+
+rnntStatus_t rnnt_b200_pruned_backward_ex(int dtype, const void* activations, void* gradients, const int* ranges,
+                                          int s_range, const int* flat_labels, const int* label_lengths,
+                                          const int* input_lengths, int alphabet_size, int minibatch,
+                                          const void* grad_costs_device, double grad_scale,
+                                          rnntGradOptions grad_options, void* workspace, rnntOptions options) {
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
+    c.pruned = true;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options, ranges, s_range}, c);
+}
+
+rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const int* input_lengths, int minibatch,
+                                              int s_range, int* ranges, const void* workspace, rnntOptions options) {
+    const int T = options.maxT, U = options.maxU, N = minibatch;
+    if (!label_lengths || !input_lengths || !ranges || !workspace || N <= 0 || T <= 0 || U <= 0 || s_range < 2)
+        return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU || (uint64_t)N * T * U >= (1ull << 31) || U > 1024) return RNNT_STATUS_INVALID_VALUE;
+    const size_t smem = prune_ranges_smem(T, U);
+    int dev = 0, optin = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+        smem > (size_t)optin)
+        return RNNT_STATUS_INVALID_VALUE;   // maxT beyond ~50k frames: the window starts no longer fit on chip
+    if (smem > 48 * 1024)
+        func_attr_once(reinterpret_cast<const void*>(joint_prune_ranges_kernel),
+                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const JointWorkspace w = carve_joint(const_cast<void*>(workspace), N, T, U, 1);   // lattice sections: V-free
+    Tensors t{nullptr, nullptr, nullptr, label_lengths, input_lengths, 1, N, nullptr, nullptr, options};
+    joint_prune_ranges_kernel<<<N, kRangeWarps * 32, smem, reinterpret_cast<cudaStream_t>(options.stream)>>>(
+        w.lp2, w.alphas, w.betas, w.llf, input_lengths, label_lengths, ranges, make_dims(t, false), s_range);
+    g_last_launches = 1;
+    return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED;
 }
 
 rnntStatus_t get_workspace_size(int maxT, int maxU, int minibatch, bool gpu, size_t* size_bytes,

@@ -261,6 +261,77 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
     Lb[r] = lb;
 }
 
+// ---- pruning ranges (DESIGN.md §8) from the lattice a forward with beta left in the workspace ---------------
+// With E = max(U_b - R, 0) and the occupancies  e_b(t,u) = exp(alpha(t,u) + lp_blank(t,u) + beta(t+1,u) - ll),
+// e_y(t,u) = exp(alpha(t,u) + lp_y(t,u) + beta(t,u+1) - ll):
+//   1. 0 < t < T_b - 1: s[t] = the smallest a in [0, E] maximising
+//      sum_{u=a}^{min(a+R,U_b)-1} e_b(t,u) - [a>0] e_y(t,a-1)
+//   2. s[0] = 0; s[T_b-1] = E if T_b > 1; s[t] = E for t >= T_b
+//   3. t = T_b-2 down to 0: s[t] = min(max(s[t], s[t+1] - (R-1)), s[t+1])
+// One CTA per utterance.  A warp takes a frame at a time: the frame's occupancies go to the warp's shared-memory
+// rows, lane l scores the starts a = l, l+32, ... (strict > keeps its smallest best) and a shuffle argmax keeps the
+// smallest a on ties.  Thread 0 then runs the sweep over the frame starts in shared memory.
+constexpr int kRangeWarps = 4;
+inline size_t prune_ranges_smem(int maxT, int maxU) {
+    return (size_t)kRangeWarps * 2 * maxU * sizeof(float) + (size_t)maxT * sizeof(int);
+}
+__global__ void __launch_bounds__(kRangeWarps * 32)
+joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                          const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                          const int* __restrict__ xlen, const int* __restrict__ ylen, int* __restrict__ ranges,
+                          const Dims d, const int R) {
+    extern __shared__ float range_smem[];   // [kRangeWarps][2][maxU] occupancies, then [maxT] window starts
+    const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int Tb, Ub;
+    utt_extent(d, xlen, ylen, b, Tb, Ub);
+    const int E = max(Ub - R, 0);
+    float* eb = range_smem + (size_t)warp * 2 * d.maxU;
+    float* ey = eb + d.maxU;
+    int* s = reinterpret_cast<int*>(range_smem + (size_t)kRangeWarps * 2 * d.maxU);
+    const LogVal ll = llf[b];
+    for (int t = 1 + warp; t < Tb - 1; t += kRangeWarps) {
+        for (int u = lane; u < Ub; u += 32) {
+            // exp2 domain, as joint_weights_kernel: exact integer exponent + small float part
+            const float4 fc = lp2[skew(d, b, t, u)];
+            const size_t q = cell(d, b, t, u);
+            const LogVal a = alphas[q], bn = betas[q + d.maxU];
+            const int oe = a.e - ll.e;
+            const float ol = a.l - ll.l;
+            eb[u] = exp2f((float)(oe + bn.e) + (ol + bn.l) + ((float)__float_as_int(fc.y) + log2f(fc.x)));
+            if (u < Ub - 1) {
+                const LogVal bl = betas[q + 1];
+                ey[u] = exp2f((float)(oe + bl.e) + (ol + bl.l) + ((float)__float_as_int(fc.w) + log2f(fc.z)));
+            }
+        }
+        __syncwarp();
+        float best = -INFINITY;
+        int best_a = E;
+        for (int a = lane; a <= E; a += 32) {
+            float sc = 0.0f;
+            const int end = min(a + R, Ub);
+            for (int u = a; u < end; ++u) sc += eb[u];
+            if (a > 0) sc -= ey[a - 1];
+            if (sc > best) best = sc, best_a = a;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oa = __shfl_xor_sync(0xffffffffu, best_a, o);
+            if (ob > best || (ob == best && oa < best_a)) best = ob, best_a = oa;
+        }
+        if (lane == 0) s[t] = best_a;
+        __syncwarp();   // the rows are rewritten for the warp's next frame
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        s[0] = 0;
+        if (Tb > 1) s[Tb - 1] = E;
+        for (int t = Tb - 2; t >= 0; --t) s[t] = min(max(s[t], s[t + 1] - (R - 1)), s[t + 1]);
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < d.maxT; t += blockDim.x) ranges[(size_t)b * d.maxT + t] = t < Tb ? s[t] : E;
+}
+
 // ---- J4/J5: out[b,r,v] = Eout[b,r,v] * sum_s W(r,s) * Ein[b,s,v]  (thin contraction over s) ----------
 //   dF: r = t, s = u, W(r,s) = Wm[b,t,u], Ein = Eg, Eout = Ef
 //   dG: r = u, s = t, W(r,s) = Wm[b,t,u] (transposed access), Ein = Ef, Eout = Eg

@@ -114,3 +114,7 @@ class RNNTLoss(Module):
 
 
 from ._checks import certify_inputs, check_contiguous, check_dim, check_type  # noqa: E402,F401
+from .pruned import (PrunedRNNTLoss, add_joint_rnnt_loss_with_ranges, prune_joint_inputs,  # noqa: E402
+                     pruned_rnnt_loss)
+
+__all__ += ['pruned_rnnt_loss', 'PrunedRNNTLoss', 'add_joint_rnnt_loss_with_ranges', 'prune_joint_inputs']

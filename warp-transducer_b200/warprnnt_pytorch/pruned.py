@@ -1,0 +1,237 @@
+"""Pruned RNN-T loss (Kuang et al., "Pruned RNN-T for fast, memory-efficient ASR training", Interspeech 2022),
+with the pruning ranges taken from the additive joint's lattice (DESIGN.md §8).
+
+A training step with a real (nonlinear) joiner:
+
+    simple, ranges = add_joint_rnnt_loss_with_ranges(am_proj, lm_proj, labels, act_lens, label_lens, s_range=5)
+    enc_p, dec_p = prune_joint_inputs(enc, dec, ranges, s_range=5)          # [N,T,R,D] each
+    logits = joiner(enc_p, dec_p)                                             # [N,T,R,V]
+    pruned = pruned_rnnt_loss(logits, labels, act_lens, label_lens, ranges)
+    (simple_scale * simple + pruned).backward()
+
+The pruned loss reads R logits per frame instead of U: row (b, t, s) of `logits` is lattice cell
+(t, ranges[b, t] + s).  Cells no row covers cannot be visited; rows outside the utterance get a zero gradient.
+"""
+import ctypes as C
+
+import torch
+from torch.autograd import Function
+from torch.nn import Module
+
+from . import warp_rnnt
+from ._checks import LengthCheck, check_contiguous, check_dim, check_type
+from .joint import _AddJointRNNT, _joint_opts, _lab_ptr, certify_joint_inputs
+
+_lib = warp_rnnt.lib()
+_P = C.c_void_p
+_Opt, _GOpt = warp_rnnt.rnntOptions, warp_rnnt.rnntGradOptions
+_lib.rnnt_b200_pruned_workspace_size.restype = C.c_int
+_lib.rnnt_b200_pruned_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t,
+                                                 C.POINTER(C.c_size_t)]
+_lib.rnnt_b200_pruned_loss_async_ex.restype = C.c_int
+_lib.rnnt_b200_pruned_loss_async_ex.argtypes = [C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int,
+                                                _P, C.c_double, _GOpt, _P, _Opt]
+_lib.rnnt_b200_pruned_forward.restype = C.c_int
+_lib.rnnt_b200_pruned_forward.argtypes = [C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, _P,
+                                          _Opt]
+_lib.rnnt_b200_pruned_backward_ex.restype = C.c_int
+_lib.rnnt_b200_pruned_backward_ex.argtypes = [C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P,
+                                              C.c_double, _GOpt, _P, _Opt]
+_lib.rnnt_b200_add_joint_prune_ranges.restype = C.c_int
+_lib.rnnt_b200_add_joint_prune_ranges.argtypes = [_P, _P, C.c_int, C.c_int, _P, _P, _Opt]
+_lib.rnnt_b200_add_joint_workspace_size.restype = C.c_int
+
+
+def pruned_workspace_size(maxT, maxU, s_range, minibatch, dtype_size=4):
+    n = C.c_size_t(0)
+    st = _lib.rnnt_b200_pruned_workspace_size(maxT, maxU, s_range, minibatch, dtype_size, C.byref(n))
+    if st != 0:
+        raise ValueError("rnnt_b200_pruned_workspace_size: " + warp_rnnt.status_string(st))
+    return n.value
+
+
+# ---- pruning ranges from the additive joint -------------------------------------------------------------------
+class _AddJointRNNTRanges(Function):
+    """_AddJointRNNT's forward with beta always kept, plus the ranges kernel on its workspace; the same backward."""
+
+    @staticmethod
+    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, s_range):
+        gopt = warp_rnnt.grad_options(fastemit_lambda)   # ValueError before any device work
+        if gopt is not None:
+            gopt.clamp = 0.0
+        s_range = int(s_range)
+        if s_range < 2:
+            raise ValueError("s_range must be >= 2, got %d" % s_range)
+        length_check = certify_joint_inputs(trans, pred, labels, act_lens, label_lens, defer=True)
+        if not trans.is_cuda:
+            raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only")
+        warp_rnnt.require_same_device(trans, pred=pred, labels=labels, act_lens=act_lens, label_lens=label_lens)
+        if reduction not in ('none', 'sum', 'mean'):
+            raise ValueError("reduction must be 'none', 'sum' or 'mean'")
+        N, T, V = trans.shape
+        U = pred.shape[1]
+        length_check.guard_labels(labels, N)
+        costs = torch.empty(N, dtype=torch.float32, device=trans.device)
+        ranges = torch.empty((N, T), dtype=torch.int32, device=trans.device)
+        n = C.c_size_t(0)
+        _lib.rnnt_b200_add_joint_workspace_size(T, U, N, V, C.byref(n))
+        with torch.cuda.device(trans.device):
+            ws = torch.empty(n.value, dtype=torch.uint8, device=trans.device)
+            opts = _joint_opts(trans, pred, blank)
+            st = _lib.rnnt_b200_add_joint_forward(trans.data_ptr(), pred.data_ptr(), _lab_ptr(labels),
+                                                  label_lens.data_ptr(), act_lens.data_ptr(), V, N,
+                                                  costs.data_ptr(), 1, ws.data_ptr(), opts)
+            if st != 0:
+                raise RuntimeError("rnnt_b200_add_joint_forward failed: " + warp_rnnt.status_string(st))
+            st = _lib.rnnt_b200_add_joint_prune_ranges(label_lens.data_ptr(), act_lens.data_ptr(), N, s_range,
+                                                       ranges.data_ptr(), ws.data_ptr(), opts)
+        if st != 0:
+            raise RuntimeError("rnnt_b200_add_joint_prune_ranges failed: " + warp_rnnt.status_string(st))
+        length_check.finish()
+        ctx.mark_non_differentiable(ranges)
+        ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
+        ctx.ws, ctx.blank, ctx.gopt = ws, blank, gopt
+        ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
+        if reduction in ('sum', 'mean'):
+            costs = costs.sum().unsqueeze_(-1)
+            if reduction == 'mean':
+                costs /= N
+        return costs, ranges
+
+    @staticmethod
+    def backward(ctx, grad_output, grad_ranges):
+        dtrans, dpred = _AddJointRNNT.backward(ctx, grad_output)[:2]
+        return dtrans, dpred, None, None, None, None, None, None, None
+
+
+def add_joint_rnnt_loss_with_ranges(trans, pred, labels, act_lens, label_lens, s_range, blank=0, reduction='mean',
+                                    *, fastemit_lambda=0.0):
+    """(loss, ranges): add_joint_rnnt_loss (the "simple" loss of pruned RNN-T; differentiable in trans and pred
+    exactly as add_joint_rnnt_loss) and the [N, T] int32 window starts of the pruned loss for R = s_range >= 2,
+    from the same forward (include/rnnt.h, rnnt_b200_add_joint_prune_ranges, defines them)."""
+    return _AddJointRNNTRanges.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
+                                     s_range)
+
+
+def prune_joint_inputs(enc, dec, ranges, s_range):
+    """The joiner's inputs at the pruned cells: enc [N,T,D] expanded (no copy) and dec [N,U,D] gathered at
+    clamp(ranges + s, 0, U-1), both [N, T, s_range, D].  Rows whose u is clamped are padding to the pruned loss, so
+    what they hold does not matter.  (k2's do_rnnt_pruning, torch only.)"""
+    N, T, D = enc.shape
+    U = dec.shape[1]
+    R = int(s_range)
+    if ranges.shape != (N, T):
+        raise ValueError("ranges must be [N, T] = [%d, %d], got %s" % (N, T, tuple(ranges.shape)))
+    idx = (ranges.long().unsqueeze(-1) + torch.arange(R, device=ranges.device)).clamp_(0, U - 1)   # [N,T,R]
+    dec_p = torch.gather(dec.unsqueeze(1).expand(N, T, U, D), 2, idx.unsqueeze(-1).expand(N, T, R, D))
+    return enc.unsqueeze(2).expand(N, T, R, D), dec_p
+
+
+# ---- pruned loss ------------------------------------------------------------------------------------------------
+def _check_pruned_inputs(logits, labels, act_lens, label_lens, ranges):
+    """RNNTLoss's input rules for [N, T, R, V] logits (U comes from labels), plus the ranges."""
+    named = (("logits", logits, None, 4), ("labels", labels, torch.int32, 2),
+             ("lengths", act_lens, torch.int32, 1), ("label_lengths", label_lens, torch.int32, 1),
+             ("ranges", ranges, torch.int32, 2))
+    for name, tensor, dtype, _ in named:
+        if dtype is not None:
+            check_type(tensor, dtype, name)
+    for name, tensor, _, _ in named:
+        check_contiguous(tensor, name)
+    for name, tensor, _, rank in named:
+        check_dim(tensor, rank, name)
+    N, T = logits.shape[0], logits.shape[1]
+    if act_lens.shape[0] != N:
+        raise ValueError("must have a length per example.")
+    if label_lens.shape[0] != N:
+        raise ValueError("must have a label length per example.")
+    if tuple(ranges.shape) != (N, T):
+        raise ValueError("ranges must be [N, T] = [%d, %d], got %s" % (N, T, tuple(ranges.shape)))
+    if not logits.is_cuda:
+        raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only; there is no CPU fallback")
+    warp_rnnt.require_same_device(logits, labels=labels, act_lens=act_lens, label_lens=label_lens, ranges=ranges)
+    return LengthCheck(act_lens, label_lens, T, labels.shape[1] + 1)
+
+
+def _opts(logits, blank, maxU):
+    return _Opt(loc=1, num_threads=0, stream=torch.cuda.current_stream(logits.device).cuda_stream,
+                blank_label=blank, maxT=logits.shape[1], maxU=maxU, batch_first=True)
+
+
+class _PrunedRNNT(Function):
+    """_RNNT's split for [N, T, R, V] logits: forward = statistics of the rows + the pruned lattices, backward =
+    the gradient pass with grad_output and the 'mean' factor folded in."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda=0.0,
+                clamp=-1.0):
+        warp_rnnt.grad_options(fastemit_lambda, clamp)   # ValueError before any device work
+        code = warp_rnnt._dtype_code(logits)
+        if reduction not in ('none', 'sum', 'mean'):
+            raise ValueError("reduction must be 'none', 'sum' or 'mean'")
+        length_check = _check_pruned_inputs(logits, labels, act_lens, label_lens, ranges)
+        N, T, R, V = logits.shape
+        U = labels.shape[1] + 1
+        length_check.guard_labels(labels, N)
+        need_grad = logits.requires_grad
+        costs = torch.empty(N, dtype=warp_rnnt.costs_dtype(logits), device=logits.device)
+        with torch.cuda.device(logits.device):
+            ws = torch.empty(pruned_workspace_size(T, U, R, N, 8 if logits.dtype == torch.float64 else 4),
+                             dtype=torch.uint8, device=logits.device)
+            st = _lib.rnnt_b200_pruned_forward(code, logits.data_ptr(), ranges.data_ptr(), R, _lab_ptr(labels),
+                                               label_lens.data_ptr(), act_lens.data_ptr(), V, N, costs.data_ptr(),
+                                               1 if need_grad else 0, ws.data_ptr(), _opts(logits, blank, U))
+        if st != 0:
+            raise RuntimeError("rnnt_b200_pruned_forward failed: " + warp_rnnt.status_string(st))
+        length_check.finish()
+        if need_grad:
+            ctx.save_for_backward(logits, labels, act_lens, label_lens, ranges)
+            ctx.workspace, ctx.blank, ctx.maxU = ws, blank, U
+            ctx.fastemit_lambda, ctx.clamp = fastemit_lambda, clamp
+            ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
+        if reduction in ('sum', 'mean'):
+            costs = costs.sum().unsqueeze_(-1)
+            if reduction == 'mean':
+                costs /= N
+        return costs
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        logits, labels, act_lens, label_lens, ranges = ctx.saved_tensors
+        N, T, R, V = logits.shape
+        g = grad_output.reshape(-1).to(device=logits.device, dtype=warp_rnnt.costs_dtype(logits))
+        g = g.expand(N).contiguous() if g.numel() == 1 else g.contiguous()
+        grads = torch.empty_like(logits)   # the kernel defines every element (zeros on padding)
+        gopt = warp_rnnt._ex_options(ctx.fastemit_lambda, ctx.clamp)
+        with torch.cuda.device(logits.device):
+            st = _lib.rnnt_b200_pruned_backward_ex(warp_rnnt._dtype_code(logits), logits.data_ptr(), grads.data_ptr(),
+                                                   ranges.data_ptr(), R, _lab_ptr(labels), label_lens.data_ptr(),
+                                                   act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale, gopt,
+                                                   ctx.workspace.data_ptr(), _opts(logits, ctx.blank, ctx.maxU))
+        if st != 0:
+            raise RuntimeError("rnnt_b200_pruned_backward_ex failed: " + warp_rnnt.status_string(st))
+        return grads, None, None, None, None, None, None, None, None
+
+
+def pruned_rnnt_loss(logits, labels, act_lens, label_lens, ranges, blank=0, reduction='mean', *,
+                     fastemit_lambda=0.0, clamp=-1.0):
+    """Pruned RNN-T loss of logits [N, T, R, V] (fp32 / fp64 / bf16 / fp16), row (b, t, s) = lattice cell
+    (t, ranges[b, t] + s); ranges [N, T] int32 on the logits' device.  labels, lengths, reduction and the gradient
+    options are rnnt_loss's; the lattice is [T, max(label_lens) + 1] as there.  An utterance whose windows leave no
+    path costs +inf with a zero gradient.  With R = U and ranges == 0 this is rnnt_loss exactly."""
+    return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda, clamp)
+
+
+class PrunedRNNTLoss(Module):
+    """Module form of pruned_rnnt_loss: PrunedRNNTLoss(blank=0, reduction='mean', *, fastemit_lambda=0.0,
+    clamp=-1.0)(logits, labels, act_lens, label_lens, ranges)."""
+
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0):
+        super().__init__()
+        warp_rnnt.grad_options(fastemit_lambda, clamp)
+        self.blank, self.reduction = blank, reduction
+        self.fastemit_lambda, self.clamp = fastemit_lambda, clamp
+
+    def forward(self, logits, labels, act_lens, label_lens, ranges):
+        return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, self.blank, self.reduction,
+                                 self.fastemit_lambda, self.clamp)
