@@ -307,6 +307,46 @@ rnntStatus_t rnnt_b200_add_joint_backward_ex(const float* trans, const float* pr
                                              void* workspace, struct rnntOptions options);
 
 /*
+ * Smoothed additive joint (DESIGN.md §9; k2's rnnt_loss_smoothed): the lattice of rnnt_b200_add_joint_forward, with
+ * each blank / label factor of a valid cell (t, u), k in {blank, y_u}, replaced by
+ *     lp(t,u,k) = c (f[t,k] + g[u,k] - lse(t,u)) + lm_only_scale (g[u,k] - Lg(u)) + am_only_scale (f[t,k] + log ug[k] - La(t))
+ * with c = 1 - lm_only_scale - am_only_scale; a term whose scale is exactly 0 is left out.
+ *   Lg(u) = log sum_v exp(g[u,v])                          the lm-only (per label position) normaliser
+ *   ug[v] = (1/M) sum_{b, u < U_b} softmax(g[b,u])[v] + FLT_MIN,  M = sum_b U_b   (valid rows of the whole batch)
+ *   La(t) = log sum_v exp(f[t,v]) ug[v]                    the am-only normaliser
+ * The gradients are the exact gradients of the returned cost in trans and pred, including the path through ug: with
+ * am_only_scale > 0 one utterance's grad_pred depends on the whole batch.  FastEmit scales the gradient of each
+ * (interpolated) label factor by 1 + fastemit_lambda.  Padded rows of pred are not read and get a zero gradient.
+ * Valid scales are finite, >= 0, with lm_only_scale + am_only_scale <= 1 + 2^-23 (one float32 ulp of slack, so
+ * that pairs meant to sum to 1, such as (0.6f, 0.4f), are accepted; c is then 0); anything else returns
+ * RNNT_STATUS_INVALID_VALUE before any device access.  Both scales 0 is the plain joint, bitwise.
+ * The smoothed workspace is the plain joint's followed by the smoothing sections, so rnnt_b200_add_joint_prune_ranges
+ * works on it as is (the windows of the smoothed lattice).  The backward half must get the scales its forward got.
+ */
+struct rnntSmoothOptions {
+    float lm_only_scale;
+    float am_only_scale;
+};
+#ifndef __cplusplus
+typedef struct rnntSmoothOptions rnntSmoothOptions;
+#endif
+rnntStatus_t rnnt_b200_add_joint_smoothed_workspace_size(int maxT, int maxU, int minibatch, int alphabet_size,
+                                                         size_t* size_bytes);
+rnntStatus_t rnnt_b200_add_joint_smoothed_forward(const float* trans, const float* pred, const int* flat_labels,
+                                                  const int* label_lengths, const int* input_lengths,
+                                                  int alphabet_size, int minibatch, float* costs_device,
+                                                  int prepare_backward, struct rnntSmoothOptions smooth,
+                                                  void* workspace, struct rnntOptions options);
+/* Gradient options as rnnt_b200_add_joint_backward_ex (FastEmit only; a nonzero clamp is INVALID_VALUE). */
+rnntStatus_t rnnt_b200_add_joint_smoothed_backward(const float* trans, const float* pred, float* grad_trans,
+                                                   float* grad_pred, const int* flat_labels,
+                                                   const int* label_lengths, const int* input_lengths,
+                                                   int alphabet_size, int minibatch, const float* grad_costs_device,
+                                                   float grad_scale, struct rnntGradOptions grad_options,
+                                                   struct rnntSmoothOptions smooth, void* workspace,
+                                                   struct rnntOptions options);
+
+/*
  * Pruned RNN-T loss (Kuang et al., "Pruned RNN-T for fast, memory-efficient ASR training", Interspeech 2022).
  * activations [minibatch, maxT, s_range, alphabet_size]: row (b, t, s) holds the logits of lattice cell
  * (t, u = ranges[b*maxT + t] + s); ranges [minibatch, maxT] int32 window starts (any values); labels, lengths and

@@ -268,6 +268,14 @@ inline bool grad_options_valid(const rnntGradOptions& o) {
     return std::isfinite(o.fastemit_lambda) && o.fastemit_lambda >= 0.0f && !std::isnan(o.clamp);
 }
 inline bool grad_options_on(const rnntGradOptions& o) { return o.fastemit_lambda > 0.0f || o.clamp > 0.0f; }
+// smoothing scales of the additive joint (include/rnnt.h rnntSmoothOptions)
+// The sum may exceed 1 by one float32 ulp of 1: scales the caller chose to sum to exactly 1, such as (0.6, 0.4),
+// arrive rounded to float32 and can sum to 1 + 3e-8 (c then becomes 0).
+inline bool smooth_valid(const rnntSmoothOptions& o) {
+    const double l = o.lm_only_scale, a = o.am_only_scale;
+    return std::isfinite(l) && std::isfinite(a) && l >= 0.0 && a >= 0.0 && l + a <= 1.0 + 0x1p-23;
+}
+inline bool smooth_on(const rnntSmoothOptions& o) { return o.lm_only_scale != 0.0f || o.am_only_scale != 0.0f; }
 template <typename T> GradReg<T> make_grad_reg(const rnntGradOptions& o, const Workspace& w) {
     GradReg<T> r;
     r.lp2 = static_cast<const typename Lat<T>::fac*>(w.lp2);
@@ -293,6 +301,7 @@ struct Call {
     const void* scale_vec;   // per-utterance gradient multipliers in the arithmetic type, or NULL
     rnntGradOptions grad;
     bool pruned = false;     // logits [N,maxT,R,V] over the windows Tensors::ranges (DESIGN.md §8)
+    rnntSmoothOptions smooth = {0.0f, 0.0f};   // additive joint: lm-only / am-only scales (DESIGN.md §9)
 };
 Call full_call(double scale, bool async = true, bool tunv = false, rnntGradOptions grad = {0.0f, 0.0f}) {
     return Call{kFull, async, false, tunv, scale, nullptr, grad};
@@ -321,7 +330,7 @@ struct Tensors {
 // The checks of every compute call, all before any device access; the first that fails decides the status.
 rnntStatus_t check_call(const Tensors& t, const Call& c) {
     const rnntOptions& opt = t.opt;
-    if (!grad_options_valid(c.grad)) return RNNT_STATUS_INVALID_VALUE;
+    if (!grad_options_valid(c.grad) || !smooth_valid(c.smooth)) return RNNT_STATUS_INVALID_VALUE;
     if (!t.acts || !t.labels || !t.ylen || !t.xlen || (!t.costs && c.phase != kBackward) || !t.workspace ||
         t.V <= 0 || t.N <= 0 || opt.maxT <= 0 || opt.maxU <= 0 || (c.phase == kBackward && !t.grads))
         return RNNT_STATUS_INVALID_VALUE;  // reference src/rnnt_entrypoint.cpp:49-59
@@ -872,9 +881,13 @@ struct JointWorkspace {
     float *ef, *eg, *mf, *mg, *inv_s, *wm, *bk, *lb, *part;
     float4* lp2;
     LogVal *alphas, *betas, *llf, *llb;
+    // smoothing sections (DESIGN.md §9), after the plain ones: carved only for a smoothed workspace
+    float *sg, *A, *ug, *lug, *msum, *amw, *ou, *bu, *lu, *h;
+    double* cpart;
+    float2 *coef_f, *coef_g;
     size_t bytes;
 };
-JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
+JointWorkspace carve_joint(void* base, int N, int T, int U, int V, bool smooth = false) {
     JointWorkspace w;
     Carver c(base);
     const size_t C = (size_t)N * T * U, D = (size_t)N * (T + U - 1) * U;
@@ -893,6 +906,22 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
     w.bk = c.take<float>(C * 4);
     w.lb = c.take<float>(C * 4);
     w.part = c.take<float>(C * 4 * kJointSlices);
+    if (smooth) {
+        const size_t NT = (size_t)N * T, NU = (size_t)N * U;
+        w.sg = c.take<float>(NU * 4);
+        w.A = c.take<float>(NT * 4);
+        w.ug = c.take<float>((size_t)V * 4);
+        w.lug = c.take<float>((size_t)V * 4);
+        w.msum = c.take<float>(4);
+        w.amw = c.take<float>(NT * 4);
+        w.ou = c.take<float>(NU * 4);
+        w.bu = c.take<float>(NU * 4);
+        w.lu = c.take<float>(NU * 4);
+        w.h = c.take<float>((size_t)V * 4);
+        w.cpart = c.take<double>((size_t)kSmoothChunks * V * 8);
+        w.coef_f = c.take<float2>(NT * 8);
+        w.coef_g = c.take<float2>(NU * 8);
+    }
     w.bytes = c.off + 256;
     return w;
 }
@@ -900,17 +929,27 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V) {
 // ---- tensor-core contractions of the additive joint (rnnt_wgmma.cuh) ---------------------------------
 // N (accumulator columns per CTA) is the smallest instantiated width that holds `n`, tiled beyond 128
 // (a thread holds N/2 accumulators: 128 columns keep two CTAs of 256 threads resident per SM).
-template <int A_MODE, int B_MODE, int KS>
+// SMOOTH: the gradient epilogue adds the smoothing terms `sm` (DESIGN.md §9).
+template <int A_MODE, int B_MODE, int KS, bool SMOOTH = false>
 void launch_wgmma(const wg::Operand& A, const wg::Operand& B, int m, int n, int K, int slices, int batch,
-                 const wg::Epilogue& epi, cudaStream_t s, int max_tile = 128) {
-    auto go = [&](auto kernel, int NT, size_t smem) {
-        func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                 const wg::Epilogue& epi, cudaStream_t s, int max_tile = 128, const wg::Smooth& sm = wg::Smooth{}) {
+    auto go = [&](auto tile) {
+        constexpr int NT = decltype(tile)::value;
+        const size_t smem = wg::gemm_smem_bytes<NT, KS>();
         dim3 grid((unsigned)(slices * ((n + NT - 1) / NT)), (unsigned)((m + 127) / 128), (unsigned)batch);
-        kernel<<<grid, wg::kThreads, smem, s>>>(A, B, K, slices, epi);
+        if constexpr (SMOOTH) {
+            auto kernel = wg::gemm_kernel<A_MODE, B_MODE, NT, KS, wg::Smooth>;
+            func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            kernel<<<grid, wg::kThreads, smem, s>>>(A, B, K, slices, epi, sm);
+        } else {
+            auto kernel = wg::gemm_kernel<A_MODE, B_MODE, NT, KS>;
+            func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            kernel<<<grid, wg::kThreads, smem, s>>>(A, B, K, slices, epi);
+        }
     };
-    if (n <= 32) go(wg::gemm_kernel<A_MODE, B_MODE, 32, KS>, 32, wg::gemm_smem_bytes<32, KS>());
-    else if (n <= 64 || max_tile <= 64) go(wg::gemm_kernel<A_MODE, B_MODE, 64, KS>, 64, wg::gemm_smem_bytes<64, KS>());
-    else go(wg::gemm_kernel<A_MODE, B_MODE, 128, KS>, 128, wg::gemm_smem_bytes<128, KS>());
+    if (n <= 32) go(std::integral_constant<int, 32>{});
+    else if (n <= 64 || max_tile <= 64) go(std::integral_constant<int, 64>{});
+    else go(std::integral_constant<int, 128>{});
 }
 
 // t.acts / t.grads: the transcription factor f [N,T,V] and its gradient; g / dG: the prediction factor
@@ -931,26 +970,49 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
     const float fastemit_lambda = c.grad.fastemit_lambda;
     g_last_launches = 0;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(opt.stream);
-    JointWorkspace w = carve_joint(t.workspace, N, T, U, V);
+    // smoothing (DESIGN.md §9): the SMOOTH instantiations and the extra kernels; both scales 0 is the plain joint
+    const bool sm = smooth_on(c.smooth);
+    const float lml = c.smooth.lm_only_scale, lma = c.smooth.am_only_scale;
+    const float cfull = (float)std::max(0.0, 1.0 - (double)lml - (double)lma);
+    JointWorkspace w = carve_joint(t.workspace, N, T, U, V, sm);
     JointDims jd{N, T, U, V, opt.blank_label};
     const Dims d = make_dims(t, false);
     const bool want_grad = dF != nullptr && c.phase != kForward;
     const bool with_beta = dF != nullptr || c.want_beta;
 
     if (c.phase != kBackward) {
-    // J1: factor-wise max and exponentials
-    auto prep = [&](const float* x, float* e, float* mx, int rows) {
+    // J1: factor-wise max and exponentials (SUM: and sum[row] = sum_k e_k wv[k], wv NULL: 1)
+    auto prep = [&](auto sum, const float* x, float* e, float* mx, int rows, const float* wv = nullptr,
+                    float* rowsum = nullptr) {
+        constexpr bool SUM = decltype(sum)::value;
         const int per = (V / 4 + 255) / 256;   // float4 per thread when one CTA owns a row
         const bool vec = V % 4 == 0 && per <= 8 && V >= 1024 && reinterpret_cast<uintptr_t>(x) % 16 == 0;
-        if (!vec) joint_prep_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, e, mx, rows, V);
-        else if (per <= 1) joint_prep_row_kernel<1><<<rows, 256, 0, s>>>(x, e, mx, V);
-        else if (per <= 2) joint_prep_row_kernel<2><<<rows, 256, 0, s>>>(x, e, mx, V);
-        else if (per <= 4) joint_prep_row_kernel<4><<<rows, 256, 0, s>>>(x, e, mx, V);
-        else if (per <= 5) joint_prep_row_kernel<5><<<rows, 256, 0, s>>>(x, e, mx, V);
-        else joint_prep_row_kernel<8><<<rows, 256, 0, s>>>(x, e, mx, V);
+        if (!vec) joint_prep_kernel<SUM><<<(rows + 7) / 8, 256, 0, s>>>(x, e, mx, rows, V, wv, rowsum);
+        else if (per <= 1) joint_prep_row_kernel<1, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
+        else if (per <= 2) joint_prep_row_kernel<2, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
+        else if (per <= 4) joint_prep_row_kernel<4, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
+        else if (per <= 5) joint_prep_row_kernel<5, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
+        else joint_prep_row_kernel<8, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
     };
-    prep(f, w.ef, w.mf, N * T);
-    prep(g, w.eg, w.mg, N * U);
+    using Plain = std::false_type;
+    using Sum = std::true_type;
+    if (!sm) {
+        prep(Plain{}, f, w.ef, w.mf, N * T);
+        prep(Plain{}, g, w.eg, w.mg, N * U);
+    } else {
+        // g first (Eg and its row sums sg), then the unigram of the valid pred rows, then f (with A = Ef . ug)
+        prep(Sum{}, g, w.eg, w.mg, N * U, nullptr, w.sg);
+        if (lma != 0.0f) {
+            const int chunks = smooth_chunks(N * U);
+            joint_colsum_kernel<true><<<dim3((V + 255) / 256, chunks), 256, 0, s>>>(w.eg, w.sg, ylen, 1, N, U, V,
+                                                                                  chunks, w.cpart);
+            joint_unigram_kernel<<<(V + 255) / 256, 256, 0, s>>>(w.cpart, chunks, ylen, N, U, V, w.ug, w.lug, w.msum);
+            prep(Sum{}, f, w.ef, w.mf, N * T, w.ug, w.A);
+            g_last_launches += 2;
+        } else {
+            prep(Plain{}, f, w.ef, w.mf, N * T);
+        }
+    }
     // J2: S = Ef . Eg^T in kJointSlices deterministic K-slabs, then lse + lattice log-prob pairs
     {
         const int slices = joint_slices(V);
@@ -976,8 +1038,14 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
                     A, B, T, U, V, slices, EpiPartial{w.part, (size_t)d.rows, T, U, slices});
             }
         }
-        EpiStats epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d};
-        joint_stats_kernel<<<(d.rows + 255) / 256, 256, 0, s>>>(w.part, slices, epi);
+        if (!sm) {
+            EpiStats<> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d};
+            joint_stats_kernel<<<(d.rows + 255) / 256, 256, 0, s>>>(w.part, slices, epi);
+        } else {
+            EpiStats<true> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d, w.sg, w.A, w.lug,
+                               cfull, lml, lma};
+            joint_stats_kernel<true><<<(d.rows + 255) / 256, 256, 0, s>>>(w.part, slices, epi);
+        }
     }
     // lattice: the dense path's fp32 wavefront, with the default ring depth and no PDL
     launch_lattice_lin(w.lp2, xlen, ylen, w.alphas, w.betas, w.llf, w.llb, costs, d, with_beta, 8, s, false);
@@ -989,9 +1057,31 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
                                (uint64_t)N * T * wg::kWmPad < (1ull << 31);   // padded weights are indexed with 32 bits
         const int wm_pitch = use_fused ? wg::kWmPad : U;
         const unsigned wm_entries = (unsigned)N * T * wm_pitch;
-        auto weights = fastemit_lambda > 0.0f ? joint_weights_kernel<true> : joint_weights_kernel<false>;
+        auto weights = fastemit_lambda > 0.0f ? (sm ? joint_weights_kernel<true, true> : joint_weights_kernel<true>)
+                                              : (sm ? joint_weights_kernel<false, true> : joint_weights_kernel<false>);
         weights<<<(wm_entries + 255) / 256, 256, 0, s>>>(w.lp2, w.alphas, w.betas, w.llf, w.inv_s, xlen, ylen, w.wm, w.bk,
-                                                         w.lb, scale, scale_vec, d, wm_pitch, fastemit_lambda);
+                                                         w.lb, scale, scale_vec, d, wm_pitch, fastemit_lambda, cfull);
+        // smoothing: the per-row epilogue coefficients of dF and dG, and h (the gradient through ug) when lma > 0
+        wg::Smooth smf{}, smg{};
+        if (sm) {
+            joint_smooth_rows_kernel<<<(N * (T + U) + 7) / 8, 256, 0, s>>>(w.bk, w.lb, w.A, xlen, ylen, jd, lma,
+                                                                              w.coef_f, w.amw, w.ou, w.bu, w.lu);
+            const float* h = nullptr;
+            if (lma != 0.0f) {
+                const int chunks = smooth_chunks(N * T);
+                joint_colsum_kernel<false><<<dim3((V + 255) / 256, chunks), 256, 0, s>>>(w.ef, w.amw, xlen, 0, N, T, V,
+                                                                                       chunks, w.cpart);
+                joint_unigram_grad_kernel<<<(V + 255) / 256, 256, 0, s>>>(w.cpart, chunks, w.ug, w.bu, w.lu, labels,
+                                                                          ylen, jd, lma, w.h);
+                h = w.h;
+                g_last_launches += 2;
+            }
+            joint_smooth_g_kernel<<<(N * U + 7) / 8, 256, 0, s>>>(w.eg, w.sg, h, w.ou, w.msum, ylen, jd, lml, w.coef_g);
+            // without the am-only term the dF coefficients are zero: no smoothing term on dF at all
+            if (lma != 0.0f) smf = wg::Smooth{w.coef_f, T, w.ug};
+            smg = wg::Smooth{w.coef_g, U, h};
+            g_last_launches += 2;
+        }
         if (!hk.joint_simt) {
             // wgmma, vocabulary index on the accumulator rows (32-byte sectors in the epilogue):
             //   dF[t,v] = Ef[t,v] * sum_u Eg[u,v] Wm[t,u]      M = v, N = t, K = u
@@ -1001,47 +1091,75 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
             wg::Operand WmUT{w.wm, (long long)T * U, 1, U, U};   // (n = u, k = t): n-contiguous
             if (use_fused) {
                 // both contractions in one pass over Ef (rnnt_wgmma.cuh: grad_fused_kernel)
-                const wg::GradFused gf{w.ef, w.eg, w.wm, dF, dG, T, U, V};
+                const wg::GradFused gf{w.ef, w.eg, w.wm, dF, dG, T, U, V, smf, smg};
                 const size_t smem = wg::GradFusedGeom<32, 32>::total + hk.fused_pad_smem;   // pad: residency experiment hook
                 auto go = [&](auto kernel) {
                     func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                     kernel<<<dim3((unsigned)((V + 127) / 128), 1, (unsigned)N), wg::kThreads, smem, s>>>(gf);
                 };
-                if (V % 4 == 0) go(wg::grad_fused_kernel<32, 32, 3>);
-                else go(wg::grad_fused_kernel<32, 32, 0>);
+                if (sm) {
+                    if (V % 4 == 0) go(wg::grad_fused_kernel<32, 32, 3, true>);
+                    else go(wg::grad_fused_kernel<32, 32, 0, true>);
+                } else {
+                    if (V % 4 == 0) go(wg::grad_fused_kernel<32, 32, 3>);
+                    else go(wg::grad_fused_kernel<32, 32, 0>);
+                }
             } else {
             // dF in 64-column accumulator tiles by default: small register / shared-memory footprint -> several
             // CTAs per SM, and the whole tile's Ef fetches are in flight before the accumulator is read
             const wg::Epilogue epf{w.ef, (long long)T * V, 1, V, dF, 0, (long long)T * V, 1, V};
-            if (V % 4 == 0) launch_wgmma<3, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, hk.df_tile);   // 16-byte aligned rows
-            else launch_wgmma<0, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, hk.df_tile);
             const wg::Epilogue epg{w.eg, (long long)U * V, 1, V, dG, 0, (long long)U * V, 1, V};
-            if (V % 4 == 0) launch_wgmma<3, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
-            else launch_wgmma<0, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
+            if (!sm) {
+                if (V % 4 == 0) launch_wgmma<3, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, hk.df_tile);   // 16-byte aligned rows
+                else launch_wgmma<0, 1, 24>(EgT, WmTU, V, T, U, 1, N, epf, s, hk.df_tile);
+                if (V % 4 == 0) launch_wgmma<3, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
+                else launch_wgmma<0, 0, 24>(EfT, WmUT, V, U, T, 1, N, epg, s);
+            } else {
+                if (V % 4 == 0) launch_wgmma<3, 1, 24, true>(EgT, WmTU, V, T, U, 1, N, epf, s, hk.df_tile, smf);
+                else launch_wgmma<0, 1, 24, true>(EgT, WmTU, V, T, U, 1, N, epf, s, hk.df_tile, smf);
+                if (V % 4 == 0) launch_wgmma<3, 0, 24, true>(EfT, WmUT, V, U, T, 1, N, epg, s, 128, smg);
+                else launch_wgmma<0, 0, 24, true>(EfT, WmUT, V, U, T, 1, N, epg, s, 128, smg);
+            }
             }
         } else if (V >= 512) {  // long vocabulary: one thread per column, thin contraction
             {   // dF[t,v] = Ef[t,v] * sum_u Wm[t,u] Eg[u,v]
                 dim3 grid((V + 255) / 256, (T + kJointRT - 1) / kJointRT, N);
-                joint_thin_kernel<<<grid, 256, 0, s>>>(w.wm, U, 1, (size_t)T * U, w.eg, w.ef, dF, T, U, V);
+                if (!sm) joint_thin_kernel<<<grid, 256, 0, s>>>(w.wm, U, 1, (size_t)T * U, w.eg, w.ef, dF, T, U, V,
+                                                                nullptr, nullptr);
+                else joint_thin_kernel<true><<<grid, 256, 0, s>>>(w.wm, U, 1, (size_t)T * U, w.eg, w.ef, dF, T, U, V,
+                                                                  smf.coef, smf.w);
             }
             {   // dG[u,v] = Eg[u,v] * sum_t Wm[t,u] Ef[t,v]
                 dim3 grid((V + 255) / 256, (U + kJointRT - 1) / kJointRT, N);
-                joint_thin_kernel<<<grid, 256, 0, s>>>(w.wm, 1, U, (size_t)T * U, w.ef, w.eg, dG, U, T, V);
+                if (!sm) joint_thin_kernel<<<grid, 256, 0, s>>>(w.wm, 1, U, (size_t)T * U, w.ef, w.eg, dG, U, T, V,
+                                                                nullptr, nullptr);
+                else joint_thin_kernel<true><<<grid, 256, 0, s>>>(w.wm, 1, U, (size_t)T * U, w.ef, w.eg, dG, U, T, V,
+                                                                  smg.coef, smg.w);
             }
         } else {  // short vocabulary: tiled GEMM
             {
                 Operand A{w.wm, (size_t)T * U, U, 1}, B{w.eg, (size_t)U * V, 1, V};
                 dim3 grid((V + 63) / 64, (T + 63) / 64, N);
-                joint_gemm_kernel<EpiGrad><<<grid, 256, 0, s>>>(A, B, T, V, U, 1, EpiGrad{w.ef, dF, T, V});
+                if (!sm) joint_gemm_kernel<EpiGrad<>><<<grid, 256, 0, s>>>(A, B, T, V, U, 1, EpiGrad<>{w.ef, dF, T, V});
+                else joint_gemm_kernel<EpiGrad<true>><<<grid, 256, 0, s>>>(
+                    A, B, T, V, U, 1, EpiGrad<true>{w.ef, dF, T, V, smf.coef, smf.w});
             }
             {
                 Operand A{w.wm, (size_t)T * U, 1, U}, B{w.ef, (size_t)T * V, 1, V};
                 dim3 grid((V + 63) / 64, (U + 63) / 64, N);
-                joint_gemm_kernel<EpiGrad><<<grid, 256, 0, s>>>(A, B, U, V, T, 1, EpiGrad{w.eg, dG, U, V});
+                if (!sm) joint_gemm_kernel<EpiGrad<>><<<grid, 256, 0, s>>>(A, B, U, V, T, 1, EpiGrad<>{w.eg, dG, U, V});
+                else joint_gemm_kernel<EpiGrad<true>><<<grid, 256, 0, s>>>(
+                    A, B, U, V, T, 1, EpiGrad<true>{w.eg, dG, U, V, smg.coef, smg.w});
             }
         }
-        joint_sparse_f_kernel<<<(N * T + 3) / 4, 128, 0, s>>>(dF, w.bk, w.lb, labels, ylen, jd);
-        joint_sparse_g_kernel<<<(N * U + 3) / 4, 128, 0, s>>>(dG, w.bk, w.lb, labels, xlen, ylen, jd);
+        if (!sm) {
+            joint_sparse_f_kernel<<<(N * T + 3) / 4, 128, 0, s>>>(dF, w.bk, w.lb, labels, ylen, jd, 1.0f);
+            joint_sparse_g_kernel<<<(N * U + 3) / 4, 128, 0, s>>>(dG, w.bk, w.lb, labels, xlen, ylen, jd, 1.0f);
+        } else {
+            joint_sparse_f_kernel<true><<<(N * T + 3) / 4, 128, 0, s>>>(dF, w.bk, w.lb, labels, ylen, jd, cfull + lma);
+            joint_sparse_g_kernel<true><<<(N * U + 3) / 4, 128, 0, s>>>(dG, w.bk, w.lb, labels, xlen, ylen, jd,
+                                                                        cfull + lml);
+        }
         g_last_launches += 5;
     }
     return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED;
@@ -1269,6 +1387,39 @@ rnntStatus_t rnnt_b200_add_joint_workspace_size(int maxT, int maxU, int minibatc
         return RNNT_STATUS_INVALID_VALUE;
     *size_bytes = carve_joint(nullptr, minibatch, maxT, maxU, alphabet_size).bytes;
     return RNNT_STATUS_SUCCESS;
+}
+
+// ---- smoothed additive joint (DESIGN.md §9) --------------------------------------------------------------
+rnntStatus_t rnnt_b200_add_joint_smoothed_workspace_size(int maxT, int maxU, int minibatch, int alphabet_size,
+                                                         size_t* size_bytes) {
+    if (minibatch <= 0 || maxT <= 0 || maxU <= 0 || alphabet_size <= 0 || size_bytes == nullptr)
+        return RNNT_STATUS_INVALID_VALUE;
+    *size_bytes = carve_joint(nullptr, minibatch, maxT, maxU, alphabet_size, true).bytes;
+    return RNNT_STATUS_SUCCESS;
+}
+
+rnntStatus_t rnnt_b200_add_joint_smoothed_forward(const float* trans, const float* pred, const int* flat_labels,
+                                                  const int* label_lengths, const int* input_lengths,
+                                                  int alphabet_size, int minibatch, float* costs_device,
+                                                  int prepare_backward, rnntSmoothOptions smooth, void* workspace,
+                                                  rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.smooth = smooth;
+    return run_add_joint({trans, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, pred, nullptr, c);
+}
+
+rnntStatus_t rnnt_b200_add_joint_smoothed_backward(const float* trans, const float* pred, float* grad_trans,
+                                                   float* grad_pred, const int* flat_labels,
+                                                   const int* label_lengths, const int* input_lengths,
+                                                   int alphabet_size, int minibatch, const float* grad_costs_device,
+                                                   float grad_scale, rnntGradOptions grad_options,
+                                                   rnntSmoothOptions smooth, void* workspace, rnntOptions options) {
+    if (grad_options.clamp != 0.0f) return RNNT_STATUS_INVALID_VALUE;   // as rnnt_b200_add_joint_backward_ex
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
+    c.smooth = smooth;
+    return run_add_joint({trans, grad_trans, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options}, pred, grad_pred, c);
 }
 
 // ---- pruned RNN-T loss (DESIGN.md §8): logits [N,maxT,R,V] over the windows `ranges` ---------------------

@@ -17,6 +17,7 @@
 // Limitation (documented in DESIGN.md): the factor-wise maxima bound the terms by 1 but not from
 // below; if max_k(f+g) is more than ~85 nats under mf+mg the fp32 sum underflows.
 #pragma once
+#include <float.h>
 #include "rnnt_kernels.cuh"
 #include "rnnt_lattice.cuh"
 #include "rnnt_wgmma.cuh"
@@ -29,8 +30,11 @@ struct JointDims {
 
 // ---- J1: per row of a factor: max and exp(x - max) ------------------------------------------------
 // one warp per row of V elements (rows = N*T for f, N*U for g)
+// SUM (smoothing, DESIGN.md §9): also sum[row] = sum_k e_k * wv[k] (wv NULL: 1) from the exponentials in registers
+template <bool SUM = false>
 __global__ void __launch_bounds__(256)
-joint_prep_kernel(const float* __restrict__ x, float* __restrict__ e, float* __restrict__ mx, int rows, int V) {
+joint_prep_kernel(const float* __restrict__ x, float* __restrict__ e, float* __restrict__ mx, int rows, int V,
+                  const float* __restrict__ wv, float* __restrict__ sum) {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= rows) return;
@@ -40,16 +44,28 @@ joint_prep_kernel(const float* __restrict__ x, float* __restrict__ e, float* __r
     m = group_max<32>(m);
     const float mz = (m == -INFINITY) ? 0.0f : m;
     float* q = e + (size_t)row * V;
-    for (int k = lane; k < V; k += 32) q[k] = Real<float>::exp(__ldg(p + k) - mz);
+    if (!SUM) {
+        for (int k = lane; k < V; k += 32) q[k] = Real<float>::exp(__ldg(p + k) - mz);
+    } else {
+        float sm = 0.0f;
+        for (int k = lane; k < V; k += 32) {
+            const float ek = Real<float>::exp(__ldg(p + k) - mz);
+            q[k] = ek;
+            sm = wv ? fmaf(ek, __ldg(wv + k), sm) : sm + ek;
+        }
+        sm = group_sum<32>(sm);
+        if (lane == 0) sum[row] = sm;
+    }
     if (lane == 0) mx[row] = m;
 }
 
 // Same, one CTA per row with the whole row in registers (V % 4 == 0, V <= 256*4*NV): the factor is read
 // ONCE (16-byte loads, all in flight before first use) and its exponentials written once with 16-byte
 // stores - the streaming shape of rowstats_row_kernel.
-template <int NV>
+template <int NV, bool SUM = false>
 __global__ void __launch_bounds__(256)
-joint_prep_row_kernel(const float* __restrict__ x, float* __restrict__ e, float* __restrict__ mx, int V) {
+joint_prep_row_kernel(const float* __restrict__ x, float* __restrict__ e, float* __restrict__ mx, int V,
+                      const float* __restrict__ wv, float* __restrict__ sum) {
     __shared__ float sh[8];
     const int row = blockIdx.x, nv = V >> 2;
     const float4* p = reinterpret_cast<const float4*>(x + (size_t)row * V);
@@ -70,6 +86,7 @@ joint_prep_row_kernel(const float* __restrict__ x, float* __restrict__ e, float*
     for (int w = 1; w < 8; ++w) m = fmaxf(m, sh[w]);
     const float mz = (m == -INFINITY) ? 0.0f : m;
     float4* q = reinterpret_cast<float4*>(e + (size_t)row * V);
+    float sm = 0.0f;
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
         const int i = threadIdx.x + j * 256;
@@ -80,6 +97,26 @@ joint_prep_row_kernel(const float* __restrict__ x, float* __restrict__ e, float*
             o.z = Real<float>::exp(v[j].z - mz);
             o.w = Real<float>::exp(v[j].w - mz);
             q[i] = o;
+            if (SUM) {
+                if (wv) {
+                    const float4 c = __ldg(reinterpret_cast<const float4*>(wv) + i);
+                    sm = fmaf(o.x, c.x, fmaf(o.y, c.y, fmaf(o.z, c.z, fmaf(o.w, c.w, sm))));
+                } else {
+                    sm += (o.x + o.y) + (o.z + o.w);
+                }
+            }
+        }
+    }
+    if (SUM) {   // fixed-order block sum (deterministic)
+        __shared__ float ss[8];
+        sm = group_sum<32>(sm);
+        if ((threadIdx.x & 31) == 0) ss[threadIdx.x >> 5] = sm;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            float t = ss[0];
+#pragma unroll
+            for (int w = 1; w < 8; ++w) t += ss[w];
+            sum[row] = t;
         }
     }
     if (threadIdx.x == 0) mx[row] = m;
@@ -161,6 +198,9 @@ struct EpiPartial {
 };
 
 // ---- J2 epilogue: S -> lse, lattice log-prob pair (diagonal-major), keep 1/S -----------------------
+// SMOOTH (DESIGN.md §9): each factor is  c lp_c + lml lp_l + lma lp_a  (a term with scale 0 is left out), with
+//   lp_c = f_k + g_k - lse,  lp_l = g_k - mg - log sg,  lp_a = f_k + log ug_k - mf - log A.
+template <bool SMOOTH = false>
 struct EpiStats {
     const float *f, *g, *mf, *mg;
     const int *labels, *xlen, *ylen;
@@ -168,6 +208,16 @@ struct EpiStats {
     float4* lp2;   // diagonal-major lattice factors (Lat<float>::fac)
     JointDims jd;
     Dims d;        // lattice geometry (maxT = T, maxU = U)
+    const float *sg, *A, *lug;   // SMOOTH: [N,U] row sums of Eg, [N,T] Ef . ug, [V] log ug
+    float c, lml, lma;           // SMOOTH: the three scales
+    __device__ float mix(const float* fr, const float* gr, int k, float lse, float Lg, float La) const {
+        const float fk = __ldg(fr + k), gk = __ldg(gr + k);
+        float lp = 0.0f;
+        if (c != 0.0f) lp = c * ((fk + gk) - lse);
+        if (lml != 0.0f) lp = fmaf(lml, gk - Lg, lp);
+        if (lma != 0.0f) lp = fmaf(lma, (fk + __ldg(lug + k)) - La, lp);
+        return lp;
+    }
     __device__ void operator()(int b, int t, int u, float S) const {
         int Tb, Ub;
         utt_extent(d, xlen, ylen, b, Tb, Ub);
@@ -181,9 +231,18 @@ struct EpiStats {
         inv_s[cell] = 1.0f / S;
         const float* fr = f + ((size_t)b * jd.T + t) * jd.V;
         const float* gr = g + ((size_t)b * jd.U + u) * jd.V;
+        const bool has_label = u < Ub - 1;
+        if (SMOOTH) {
+            const float Lg = mgu + logf(__ldg(sg + (size_t)b * jd.U + u));
+            const float La = lma != 0.0f ? mft + logf(__ldg(A + (size_t)b * jd.T + t)) : 0.0f;
+            const float lpb = mix(fr, gr, jd.blank, lse, Lg, La);
+            float lpl = 0.0f;
+            if (has_label) lpl = mix(fr, gr, __ldg(labels + (size_t)b * (jd.U > 1 ? jd.U - 1 : 0) + u), lse, Lg, La);
+            lp2[skew(d, b, t, u)] = make_fac(lpb, lpl, has_label);
+            return;
+        }
         const float lpb = (__ldg(fr + jd.blank) + __ldg(gr + jd.blank)) - lse;
         float lpl = 0.0f;
-        const bool has_label = u < Ub - 1;
         if (has_label) {
             const int y = __ldg(labels + (size_t)b * (jd.U > 1 ? jd.U - 1 : 0) + u);
             lpl = (__ldg(fr + y) + __ldg(gr + y)) - lse;
@@ -192,8 +251,9 @@ struct EpiStats {
     }
 };
 
+template <bool SMOOTH = false>
 __global__ void __launch_bounds__(256)
-joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats epi) {
+joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats<SMOOTH> epi) {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= epi.d.rows) return;
     uint32_t bt, u, b, t;
@@ -207,14 +267,15 @@ joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats ep
 // ---- J3: per cell weights from the lattices ---------------------------------------------------------
 //   Wm = e^{alpha+beta-ll} / S ;  Bk = blank-transition occupancy ;  Lb = label-transition occupancy
 // REG (FastEmit, rnnt_kernels.cuh GradReg): Wm += lambda Lb / S and Lb *= 1 + lambda.
-template <bool REG = false>
+// SMOOTH (DESIGN.md §9): Wm carries the scale c of the full-joint term; Bk / Lb stay the factor gradients.
+template <bool REG = false, bool SMOOTH = false>
 __global__ void __launch_bounds__(256)
 joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
                      const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
                      const float* __restrict__ inv_s, const int* __restrict__ xlen,
                      const int* __restrict__ ylen, float* __restrict__ Wm, float* __restrict__ Bk,
                      float* __restrict__ Lb, const float scale_in, const float* __restrict__ scale_vec,
-                     const Dims d, const int wm_pitch, const float lam) {
+                     const Dims d, const int wm_pitch, const float lam, const float c) {
     // Wm rows have `wm_pitch` >= maxU entries (zero beyond maxU: the tensor-core kernel fetches them as aligned
     // float4 rows); Bk / Lb / inv_s are [N,T,maxU].  One thread per Wm entry.
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -255,6 +316,7 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
                 lb *= 1.0f + lam;
             }
         }
+        if (SMOOTH) w *= c;
     }
     Wm[q] = w;
     Bk[r] = bk;
@@ -337,11 +399,14 @@ joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restri
 //   dG: r = u, s = t, W(r,s) = Wm[b,t,u] (transposed access), Ein = Ef, Eout = Eg
 // One thread per vocabulary column (coalesced over v), RT output rows per block held in registers,
 // the W tile broadcast from shared memory: RT FMAs per 4-byte load of Ein.
+// SMOOTH (DESIGN.md §9): out = Eout * (acc + coef[b,r].x + coef[b,r].y * wv[v])   (wv NULL: no last term; coef
+// NULL: no smoothing term on this product)
 constexpr int kJointRT = 16, kJointSC = 64;
+template <bool SMOOTH = false>
 __global__ void __launch_bounds__(256)
 joint_thin_kernel(const float* __restrict__ Wm, int w_stride_r, int w_stride_s, size_t w_batch,
                   const float* __restrict__ Ein, const float* __restrict__ Eout, float* __restrict__ out,
-                  int R, int S, int V) {
+                  int R, int S, int V, const float2* __restrict__ coef, const float* __restrict__ wv) {
     __shared__ float sw[kJointSC][kJointRT];
     const int b = blockIdx.z, r0 = blockIdx.y * kJointRT;
     const int v = blockIdx.x * 256 + threadIdx.x;
@@ -373,19 +438,33 @@ joint_thin_kernel(const float* __restrict__ Wm, int w_stride_r, int w_stride_s, 
             const int r = r0 + i;
             if (r < R) {
                 const size_t o = ((size_t)b * R + r) * V + v;
-                out[o] = __ldg(Eout + o) * acc[i];
+                float x = acc[i];
+                if (SMOOTH && coef) {
+                    const float2 cf = __ldg(coef + (size_t)b * R + r);
+                    x += cf.x;
+                    if (wv) x = fmaf(cf.y, __ldg(wv + v), x);
+                }
+                out[o] = __ldg(Eout + o) * x;
             }
         }
     }
 }
 
 // generic-GEMM form of the same products, used when V is too short to give every thread a column
+template <bool SMOOTH = false>
 struct EpiGrad {
     const float* e;  // Ef [N,T,V] (or Eg [N,U,V])
     float* out;      // dF (or dG), same shape
     int rows, V;     // rows per batch (T or U)
+    const float2* coef;   // SMOOTH: as joint_thin_kernel
+    const float* wv;
     __device__ void operator()(int b, int m, int n, float acc) const {
         const size_t i = ((size_t)b * rows + m) * V + n;
+        if (SMOOTH && coef) {
+            const float2 cf = __ldg(coef + (size_t)b * rows + m);
+            acc += cf.x;
+            if (wv) acc = fmaf(cf.y, __ldg(wv + n), acc);
+        }
         out[i] = e[i] * acc;
     }
 };
@@ -414,9 +493,12 @@ __device__ __forceinline__ void warp_scatter_sub(float* row, int key, float val)
     if (key >= 0 && lane == leader) row[key] -= acc;
 }
 
+// SMOOTH (DESIGN.md §9): the subtracted terms carry the factor k (c + lma on dF, c + lml on dG)
+template <bool SMOOTH = false>
 __global__ void __launch_bounds__(128)
 joint_sparse_f_kernel(float* __restrict__ dF, const float* __restrict__ Bk, const float* __restrict__ Lb,
-                      const int* __restrict__ labels, const int* __restrict__ ylen, const JointDims jd) {
+                      const int* __restrict__ labels, const int* __restrict__ ylen, const JointDims jd,
+                      const float k) {
     const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // (b,t)
     const int lane = threadIdx.x & 31;
     if (i >= jd.N * jd.T) return;
@@ -428,19 +510,21 @@ joint_sparse_f_kernel(float* __restrict__ dF, const float* __restrict__ Bk, cons
     float sb = 0.0f;
     for (int u = lane; u < Ub; u += 32) sb += bk[u];
     sb = warp_sum(sb);
-    if (lane == 0) row[jd.blank] -= sb;
+    if (lane == 0) row[jd.blank] -= SMOOTH ? k * sb : sb;
     for (int u0 = 0; u0 < Ub - 1; u0 += 32) {
         __syncwarp();
         const int u = u0 + lane;
         const bool has = u < Ub - 1;
-        warp_scatter_sub(row, has ? __ldg(labels + (size_t)b * (jd.U - 1) + u) : -1, has ? lb[u] : 0.0f);
+        warp_scatter_sub(row, has ? __ldg(labels + (size_t)b * (jd.U - 1) + u) : -1,
+                         has ? (SMOOTH ? k * lb[u] : lb[u]) : 0.0f);
     }
 }
 
+template <bool SMOOTH = false>
 __global__ void __launch_bounds__(128)
 joint_sparse_g_kernel(float* __restrict__ dG, const float* __restrict__ Bk, const float* __restrict__ Lb,
                       const int* __restrict__ labels, const int* __restrict__ xlen,
-                      const int* __restrict__ ylen, const JointDims jd) {
+                      const int* __restrict__ ylen, const JointDims jd, const float k) {
     const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // (b,u)
     const int lane = threadIdx.x & 31;
     if (i >= jd.N * jd.U) return;
@@ -457,10 +541,203 @@ joint_sparse_g_kernel(float* __restrict__ dG, const float* __restrict__ Bk, cons
     }
     sb = warp_sum(sb);
     sl = warp_sum(sl);
+    if (SMOOTH) {
+        sb *= k;
+        sl *= k;
+    }
     if (lane == 0) {
         row[jd.blank] -= sb;
         if (u < Ub - 1) row[__ldg(labels + (size_t)b * (jd.U - 1) + u)] -= sl;
     }
+}
+
+// ---- smoothing (DESIGN.md §9): the batch-wide quantities of the lm-only / am-only terms -------------------
+// Every reduction has a fixed order (fixed row chunks, fixed shuffle trees, partials summed in chunk order) and
+// no floating-point atomics, so a second call gives the same bits.
+constexpr int kSmoothChunks = 128;   // max row chunks of a column sum
+// Row chunks of a column sum over `rows` rows: at most kSmoothChunks, at least 32 rows each where there are enough,
+// and none empty (chunk c covers rows [c*per, min(rows, (c+1)*per)) with per = ceil(rows / chunks)).
+inline int smooth_chunks(int rows) {
+    const int target = rows >= 32 * kSmoothChunks ? kSmoothChunks : rows > 32 ? (rows + 31) / 32 : 1;
+    const int per = (rows + target - 1) / target;
+    return (rows + per - 1) / per;
+}
+
+// part[c][v] = sum over the VALID rows q = (b, r) of chunk c of  w(q) * E[q, v],  w(q) = INV ? 1 / wr[q] : wr[q].
+// Row r of utterance b is valid iff r < clamp(len[b] + add, 1, R); other rows are never read.  The sums are fp64:
+// the gradient through ug takes the difference h[v] - hbar of two such sums (joint_smooth_g_kernel).
+template <bool INV>
+__global__ void __launch_bounds__(256)
+joint_colsum_kernel(const float* __restrict__ E, const float* __restrict__ wr, const int* __restrict__ len, int add,
+                    int N, int R, int V, int chunks, double* __restrict__ part) {
+    const int v = blockIdx.x * 256 + threadIdx.x, c = blockIdx.y;
+    const int rows = N * R, per = (rows + chunks - 1) / chunks;
+    const int q0 = c * per, q1 = min(rows, q0 + per);
+    double acc = 0.0;
+    if (v >= V) return;
+    if (q0 < q1) {   // smooth_chunks leaves no chunk empty; the guard keeps len[] in bounds regardless
+        int b = q0 / R, r = q0 - b * R, lim = min(max(__ldg(len + b) + add, 1), R);
+        for (int q = q0; q < q1; ++q) {
+            if (r < lim) {
+                const float x = __ldg(wr + q);
+                acc += (double)((INV ? 1.0f / x : x) * __ldg(E + (size_t)q * V + v));
+            }
+            if (++r == R && q + 1 < q1) {
+                r = 0;
+                lim = min(max(__ldg(len + ++b) + add, 1), R);
+            }
+        }
+    }
+    part[(size_t)c * V + v] = acc;
+}
+
+// number of valid pred rows M = sum_b U_b (an integer sum: exact in any order)
+__device__ __forceinline__ int valid_pred_rows(const int* __restrict__ ylen, int N, int U) {
+    __shared__ int m;
+    if (threadIdx.x == 0) m = 0;
+    __syncthreads();
+    int s = 0;
+    for (int b = threadIdx.x; b < N; b += blockDim.x) s += min(max(__ldg(ylen + b) + 1, 1), U);
+    atomicAdd(&m, s);
+    __syncthreads();
+    return m;
+}
+
+// ug[v] = (1/M) sum_{valid (b,u)} Eg[b,u,v] / sg[b,u] + FLT_MIN, lug = log ug; msum[0] = M
+__global__ void __launch_bounds__(256)
+joint_unigram_kernel(const double* __restrict__ part, int chunks, const int* __restrict__ ylen, int N, int U, int V,
+                     float* __restrict__ ug, float* __restrict__ lug, float* __restrict__ msum) {
+    const float M = (float)valid_pred_rows(ylen, N, U);
+    const int v = blockIdx.x * 256 + threadIdx.x;
+    if (blockIdx.x == 0 && threadIdx.x == 0) msum[0] = M;
+    if (v >= V) return;
+    double s = 0.0;
+    for (int c = 0; c < chunks; ++c) s += part[(size_t)c * V + v];
+    const float x = (float)(s / M) + FLT_MIN;
+    ug[v] = x;
+    lug[v] = logf(x);
+}
+
+// Row totals of the factor gradients, per frame and per label position, and the dF epilogue coefficients; one warp
+// per row (fixed shuffle tree: deterministic):
+//   (b,t):  O_t = sum_u (Bk + Lb),  coefF = (0, lma O_t / A),  amw = O_t / A        (zero for t >= T_b)
+//   (b,u):  Bu = sum_t Bk,  Lu = sum_t Lb,  Ou = Bu + Lu                          (zero for u >= U_b)
+__global__ void __launch_bounds__(256)
+joint_smooth_rows_kernel(const float* __restrict__ Bk, const float* __restrict__ Lb, const float* __restrict__ A,
+                         const int* __restrict__ xlen, const int* __restrict__ ylen, const JointDims jd,
+                         const float lma, float2* __restrict__ coefF, float* __restrict__ amw,
+                         float* __restrict__ Ou, float* __restrict__ Bu, float* __restrict__ Lu) {
+    const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    const int NT = jd.N * jd.T;
+    if (q >= NT + jd.N * jd.U) return;
+    if (q < NT) {
+        const int b = q / jd.T, t = q - b * jd.T;
+        const int Tb = min(max(__ldg(xlen + b), 1), jd.T), Ub = min(max(__ldg(ylen + b) + 1, 1), jd.U);
+        float o = 0.0f, w = 0.0f;
+        if (t < Tb) {
+            const size_t c0 = (size_t)q * jd.U;
+            for (int u = lane; u < Ub; u += 32) o += Bk[c0 + u] + Lb[c0 + u];
+            o = warp_sum(o);
+            if (lma != 0.0f) w = o / __ldg(A + q);
+        }
+        if (lane == 0) {
+            coefF[q] = make_float2(0.0f, lma * w);
+            amw[q] = w;
+        }
+    } else {
+        const int i = q - NT, b = i / jd.U, u = i - b * jd.U;
+        const int Tb = min(max(__ldg(xlen + b), 1), jd.T), Ub = min(max(__ldg(ylen + b) + 1, 1), jd.U);
+        float sb = 0.0f, sl = 0.0f;
+        if (u < Ub) {
+            for (int t = lane; t < Tb; t += 32) {
+                const size_t c = ((size_t)b * jd.T + t) * jd.U + u;
+                sb += Bk[c];
+                sl += Lb[c];
+            }
+            sb = warp_sum(sb);
+            sl = warp_sum(sl);
+        }
+        if (lane == 0) {
+            Bu[i] = sb;
+            Lu[i] = sl;
+            Ou[i] = sb + sl;
+        }
+    }
+}
+
+// h[v] = lma (sum_{b,t} amw Ef[b,t,v] - Z[v] / ug[v] - K),  Z[v] = [v = blank] sum Bu + sum_{(b,u): y_u = v} Lu,
+// K = sum_{b,u} (Bu + Lu).  dG only sees h[v] - hbar_u, which a constant leaves unchanged; without K every column
+// that is no label would hold nearly the same large value, and fp32 would lose the small differences that matter.
+// The (b,u) items pass through shared memory in tiles, every thread scans them all in the same order.
+__global__ void __launch_bounds__(256)
+joint_unigram_grad_kernel(const double* __restrict__ part, int chunks, const float* __restrict__ ug,
+                          const float* __restrict__ Bu, const float* __restrict__ Lu, const int* __restrict__ labels,
+                          const int* __restrict__ ylen, const JointDims jd, const float lma, float* __restrict__ h) {
+    __shared__ int sy[256];
+    __shared__ float sb[256], sl[256];
+    const int v = blockIdx.x * 256 + threadIdx.x;
+    const int items = jd.N * jd.U;
+    double z = 0.0, K = 0.0;
+    for (int i0 = 0; i0 < items; i0 += 256) {
+        const int i = i0 + threadIdx.x;
+        int y = -1;
+        float bb = 0.0f, ll = 0.0f;
+        if (i < items) {
+            const int b = i / jd.U, u = i - b * jd.U;
+            const int Ub = min(max(__ldg(ylen + b) + 1, 1), jd.U);
+            if (u < Ub) {
+                bb = Bu[i];
+                if (u < Ub - 1) {
+                    y = __ldg(labels + (size_t)b * (jd.U - 1) + u);
+                    ll = Lu[i];
+                }
+            }
+        }
+        __syncthreads();   // the previous tile has been read
+        sy[threadIdx.x] = y;
+        sb[threadIdx.x] = bb;
+        sl[threadIdx.x] = ll;
+        __syncthreads();
+        const int n = min(256, items - i0);
+        if (v == jd.blank)
+            for (int j = 0; j < n; ++j) z += sb[j];
+        for (int j = 0; j < n; ++j) {
+            K += (double)sb[j] + (double)sl[j];
+            if (sy[j] == v) z += sl[j];
+        }
+    }
+    if (v >= jd.V) return;
+    double s = 0.0;
+    for (int c = 0; c < chunks; ++c) s += part[(size_t)c * jd.V + v];
+    h[v] = (float)(lma * (s - z / ug[v] - K));
+}
+
+// dG epilogue coefficients, one warp per (b,u):  coefG = (lml Ou / sg - hbar / (M sg), 1 / (M sg)) with
+// hbar = sum_v Eg h / sg;  without h (lma = 0): (lml Ou / sg, 0).  Zero for u >= U_b (Eg not read there).
+__global__ void __launch_bounds__(256)
+joint_smooth_g_kernel(const float* __restrict__ eg, const float* __restrict__ sg, const float* __restrict__ h,
+                      const float* __restrict__ Ou, const float* __restrict__ msum, const int* __restrict__ ylen,
+                      const JointDims jd, const float lml, float2* __restrict__ coefG) {
+    const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (i >= jd.N * jd.U) return;
+    const int b = i / jd.U, u = i - b * jd.U;
+    const int Ub = min(max(__ldg(ylen + b) + 1, 1), jd.U);
+    float2 cf = make_float2(0.0f, 0.0f);
+    if (u < Ub) {
+        const float s = __ldg(sg + i);
+        cf.x = lml * Ou[i] / s;
+        if (h) {
+            const float* row = eg + (size_t)i * jd.V;
+            double hb = 0.0;
+            for (int v = lane; v < jd.V; v += 32) hb += (double)__ldg(row + v) * (double)__ldg(h + v);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) hb += __shfl_xor_sync(0xffffffffu, hb, o);
+            const float inv = 1.0f / (__ldg(msum) * s);
+            cf.x -= (float)(hb / s) * inv;
+            cf.y = inv;
+        }
+    }
+    if (lane == 0) coefG[i] = cf;
 }
 
 }  // namespace b200rnnt

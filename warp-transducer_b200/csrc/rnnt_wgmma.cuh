@@ -379,6 +379,26 @@ struct Epilogue {
     int out_m, out_n;
 };
 
+// Smoothing terms of a gradient epilogue (DESIGN.md §9), for accumulator row m (vocabulary) and column n (t or u):
+//   acc -> acc + coef[b*coef_b + n].x + coef[b*coef_b + n].y * w[m]      (w NULL: no last term; coef NULL: acc)
+struct Smooth {
+    const float2* coef;
+    int coef_b;
+    const float* w;
+};
+template <bool SMOOTH>
+__device__ __forceinline__ float smooth_acc(float acc, const Smooth& sm, int b, int m, int n) {
+    if (!SMOOTH || !sm.coef) return acc;
+    const float2 cf = __ldg(sm.coef + (b * sm.coef_b + n));
+    acc += cf.x;
+    return sm.w ? fmaf(cf.y, __ldg(sm.w + m), acc) : acc;
+}
+// gemm_kernel's form: the smoothing terms come as an optional trailing parameter (none: the plain epilogue)
+__device__ __forceinline__ float smooth_acc_opt(float acc, int, int, int) { return acc; }
+__device__ __forceinline__ float smooth_acc_opt(float acc, int b, int m, int n, const Smooth& sm) {
+    return smooth_acc<true>(acc, sm, b, m, n);
+}
+
 // Accumulator fragment of this thread (see Mma): row and column of element i relative to the warpgroup's tile
 __device__ __forceinline__ constexpr int frag_row(int i) { return 8 * ((i >> 1) & 1); }
 __device__ __forceinline__ constexpr int frag_col(int i) { return 8 * (i >> 2) + (i & 1); }
@@ -388,9 +408,12 @@ __device__ __forceinline__ constexpr int frag_col(int i) { return 8 * (i >> 2) +
 // One shared-memory stage buffer per CTA: the footprint stays small, so several CTAs are resident per SM
 // and cover each other's load -> split -> multiply chains; within a CTA the global loads of stage s+1 are in
 // flight in registers while stage s is multiplied.  Elements with m >= A.mn_valid or n >= B.mn_valid are skipped.
-template <int A_MODE, int B_MODE, int N, int KS>
+// Sm: empty (the plain kernel, named gemm_kernel<A_MODE, B_MODE, N, KS>) or one Smooth, whose terms the epilogue
+// adds (the smoothed joint's dF / dG, DESIGN.md §9).
+template <int A_MODE, int B_MODE, int N, int KS, typename... Sm>
 __global__ void __launch_bounds__(kThreads, N <= 64 ? 3 : 2)
-gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue epi) {
+gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue epi, Sm... sm) {
+    static_assert(sizeof...(Sm) <= 1, "at most one set of smoothing terms");
     static_assert(N % 32 == 0 && N >= 32 && N <= 128 && KS % 8 == 0, "wgmma shape");
     constexpr uint32_t A_BYTES = TileGeom::bytes(128, KS), B_BYTES = TileGeom::bytes(N, KS);
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -453,10 +476,13 @@ gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue 
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) {
         const int m = m_base + frag_row(i), n = n_base + frag_col(i);
-        if (m < A.mn_valid && n < B.mn_valid)
-            op[m * epi.out_m + n * epi.out_n] = ip ? acc[i] * __ldg(ip + (m * epi.in_m + n * epi.in_n)) : acc[i];
+        if (m < A.mn_valid && n < B.mn_valid) {
+            const float x = smooth_acc_opt(acc[i], b, m, n, sm...);
+            op[m * epi.out_m + n * epi.out_n] = ip ? x * __ldg(ip + (m * epi.in_m + n * epi.in_n)) : x;
+        }
     }
 }
+
 
 // =================================================================================================
 // Both gradient contractions of the additive joint in ONE pass over Ef (the [N,T,V] factor that dominates
@@ -477,6 +503,7 @@ struct GradFused {
     const float *ef, *eg, *wm;   // [N,T,V], [N,U,V], [N,T,kWmPad]: Wm rows zero-padded to kWmPad label positions
     float *dF, *dG;              // [N,T,V], [N,U,V]
     int T, U, V;
+    Smooth sf, sg;               // SMOOTH: the dF and dG epilogue terms
 };
 constexpr int kWmPad = 32;       // the weights' row pitch (16-byte aligned rows: both Wm operands are fetched as float4)
 template <int NU, int TC> struct GradFusedGeom {
@@ -485,7 +512,7 @@ template <int NU, int TC> struct GradFusedGeom {
     static constexpr uint32_t B1 = TileGeom::bytes(TC, KU), B2 = TileGeom::bytes(NU, TC);
     static constexpr uint32_t total = 2 * (A1 + A2 + B1 + B2);
 };
-template <int NU, int TC, int A_MODE>   // A_MODE 3: rows of Ef / Eg 16-byte aligned (V % 4 == 0), else 0
+template <int NU, int TC, int A_MODE, bool SMOOTH = false>   // A_MODE 3: rows of Ef / Eg 16-byte aligned (V % 4 == 0), else 0
 __global__ void __launch_bounds__(kThreads, 2)
 grad_fused_kernel(const GradFused g) {
     static_assert(NU == 32 && TC == 32, "instantiated shape: up to 32 label positions, 32 frames per chunk");
@@ -580,7 +607,7 @@ grad_fused_kernel(const GradFused g) {
 #pragma unroll
         for (int i = 0; i < TC / 2; ++i) {
             const int v = m + frag_row(i), t = c0 + frag_col(i);
-            if (v < V && t0 + t < T) op[t * V + v] = p[i] * __ldg(ip + (t * V + v));
+            if (v < V && t0 + t < T) op[t * V + v] = smooth_acc<SMOOTH>(p[i], g.sf, b, v, t0 + t) * __ldg(ip + (t * V + v));
         }
     }
     // dG: Q is complete.  dG[u,v] = Eg[u,v] * Q[v,u]
@@ -589,7 +616,7 @@ grad_fused_kernel(const GradFused g) {
 #pragma unroll
     for (int i = 0; i < NU / 2; ++i) {
         const int v = m + frag_row(i), u = c0 + frag_col(i);
-        if (v < V && u < U) op[u * V + v] = q[i] * __ldg(ip + (u * V + v));
+        if (v < V && u < U) op[u * V + v] = smooth_acc<SMOOTH>(q[i], g.sg, b, v, u) * __ldg(ip + (u * V + v));
     }
 }
 

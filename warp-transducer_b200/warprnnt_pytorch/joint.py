@@ -10,8 +10,13 @@ Equivalent to RNNTLoss()(trans.unsqueeze(2) + pred.unsqueeze(1), ...) with gradi
 the factors, at O(N (T+U) V) memory traffic.  The keyword-only ``fastemit_lambda`` is RNNTLoss's
 FastEmit option; ``clamp`` is not available here (the factor gradients are contractions over the
 lattice, per-logit gradients never exist to be clipped) and raises ValueError.
+
+The keyword-only ``lm_only_scale`` and ``am_only_scale`` give k2's smoothed loss (rnnt_loss_smoothed, the "simple"
+loss of pruned RNN-T): every lattice factor becomes  c lp_joint + lm_only_scale lp_lm + am_only_scale lp_am  with
+c = 1 - lm_only_scale - am_only_scale (include/rnnt.h, rnntSmoothOptions; DESIGN.md §9).  Both 0 is the plain loss.
 """
 import ctypes as C
+import math
 
 import torch
 from torch.autograd import Function
@@ -36,6 +41,36 @@ _lib.rnnt_b200_add_joint_backward_ex.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c
                                                  warp_rnnt.rnntGradOptions, _P, warp_rnnt.rnntOptions]
 _lib.rnnt_b200_add_joint_workspace_size.restype = C.c_int
 _lib.rnnt_b200_add_joint_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
+
+
+class rnntSmoothOptions(C.Structure):
+    """struct rnntSmoothOptions (include/rnnt.h)."""
+    _fields_ = [("lm_only_scale", C.c_float), ("am_only_scale", C.c_float)]
+
+
+_lib.rnnt_b200_add_joint_smoothed_workspace_size.restype = C.c_int
+_lib.rnnt_b200_add_joint_smoothed_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int,
+                                                             C.POINTER(C.c_size_t)]
+_lib.rnnt_b200_add_joint_smoothed_forward.restype = C.c_int
+_lib.rnnt_b200_add_joint_smoothed_forward.argtypes = [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int,
+                                                      rnntSmoothOptions, _P, warp_rnnt.rnntOptions]
+_lib.rnnt_b200_add_joint_smoothed_backward.restype = C.c_int
+_lib.rnnt_b200_add_joint_smoothed_backward.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_float,
+                                                       warp_rnnt.rnntGradOptions, rnntSmoothOptions, _P,
+                                                       warp_rnnt.rnntOptions]
+
+
+def smooth_options(lm_only_scale=0.0, am_only_scale=0.0):
+    """Checked rnntSmoothOptions, or None when both scales are 0 (the plain entries then run).  Each scale must be
+    finite and >= 0, and their sum <= 1, as given (so (0.6, 0.4) is valid although its float32 roundings sum to
+    slightly more than 1; the C-ABI allows that one ulp)."""
+    lm0, am0 = float(lm_only_scale), float(am_only_scale)
+    if not (math.isfinite(lm0) and math.isfinite(am0) and lm0 >= 0.0 and am0 >= 0.0 and lm0 + am0 <= 1.0):
+        raise ValueError("lm_only_scale and am_only_scale must be finite, >= 0 and sum to at most 1, got %r, %r"
+                         % (lm_only_scale, am_only_scale))
+    if lm0 == 0.0 and am0 == 0.0:
+        return None
+    return rnntSmoothOptions(lm0, am0)
 
 
 def certify_joint_inputs(trans, pred, labels, lengths, label_lengths, defer=False):
@@ -94,40 +129,65 @@ def _joint_opts(trans, pred, blank):
 _lab_ptr = warp_rnnt._labels_ptr   # cached per-device stand-in when there are no labels (U == 1)
 
 
+def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare_backward, blank, smooth):
+    """The forward half on CUDA tensors (no checks): rnnt_b200_add_joint_forward, or its smoothed form when
+    `smooth` (an rnntSmoothOptions) is given.  Returns the workspace the backward half and the ranges read."""
+    N, T, V = trans.shape
+    U = pred.shape[1]
+    n = C.c_size_t(0)
+    if smooth is None:
+        _lib.rnnt_b200_add_joint_workspace_size(T, U, N, V, C.byref(n))
+    else:
+        _lib.rnnt_b200_add_joint_smoothed_workspace_size(T, U, N, V, C.byref(n))
+    ws = torch.empty(n.value, dtype=torch.uint8, device=trans.device)
+    args = (trans.data_ptr(), pred.data_ptr(), _lab_ptr(labels), label_lens.data_ptr(), act_lens.data_ptr(), V, N,
+            costs.data_ptr(), 1 if prepare_backward else 0)
+    tail = (ws.data_ptr(), _joint_opts(trans, pred, blank))
+    if smooth is None:
+        st = _lib.rnnt_b200_add_joint_forward(*args, *tail)
+    else:
+        st = _lib.rnnt_b200_add_joint_smoothed_forward(*args, smooth, *tail)
+    if st != 0:
+        raise RuntimeError("rnnt_b200_add_joint_forward failed: " + warp_rnnt.status_string(st))
+    return ws
+
+
+def check_joint_call(trans, pred, labels, act_lens, label_lens, reduction, fastemit_lambda, lm_only_scale,
+                     am_only_scale):
+    """Every argument rule of a joint call, before any device work: (gradient options, smoothing options,
+    deferred length check)."""
+    gopt = warp_rnnt.grad_options(fastemit_lambda)   # ValueError before any device work
+    if gopt is not None:
+        gopt.clamp = 0.0                              # the joint entry accepts no clamp at all
+    smooth = smooth_options(lm_only_scale, am_only_scale)
+    length_check = certify_joint_inputs(trans, pred, labels, act_lens, label_lens, defer=True)
+    if not trans.is_cuda:
+        raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only")
+    warp_rnnt.require_same_device(trans, pred=pred, labels=labels, act_lens=act_lens, label_lens=label_lens)
+    if reduction not in ('none', 'sum', 'mean'):
+        raise ValueError("reduction must be 'none', 'sum' or 'mean'")
+    return gopt, smooth, length_check
+
+
 class _AddJointRNNT(Function):
     """forward: factor exponentials, S = Ef.Eg^T, alpha/beta lattices, costs.  backward: weights +
     the two factor-gradient contractions with grad_output[b] and the reduction factor folded in."""
 
     @staticmethod
-    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0):
-        gopt = warp_rnnt.grad_options(fastemit_lambda)   # ValueError before any device work
-        if gopt is not None:
-            gopt.clamp = 0.0                              # the joint entry accepts no clamp at all
-        length_check = certify_joint_inputs(trans, pred, labels, act_lens, label_lens, defer=True)
-        if not trans.is_cuda:
-            raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only")
-        warp_rnnt.require_same_device(trans, pred=pred, labels=labels, act_lens=act_lens, label_lens=label_lens)
-        if reduction not in ('none', 'sum', 'mean'):
-            raise ValueError("reduction must be 'none', 'sum' or 'mean'")
-        N, T, V = trans.shape
-        U = pred.shape[1]
+    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0,
+                lm_only_scale=0.0, am_only_scale=0.0):
+        gopt, smooth, length_check = check_joint_call(trans, pred, labels, act_lens, label_lens, reduction,
+                                                      fastemit_lambda, lm_only_scale, am_only_scale)
+        N = trans.shape[0]
         length_check.guard_labels(labels, N)
         need = trans.requires_grad or pred.requires_grad
         costs = torch.empty(N, dtype=torch.float32, device=trans.device)
-        n = C.c_size_t(0)
-        _lib.rnnt_b200_add_joint_workspace_size(T, U, N, V, C.byref(n))
         with torch.cuda.device(trans.device):
-            ws = torch.empty(n.value, dtype=torch.uint8, device=trans.device)
-            st = _lib.rnnt_b200_add_joint_forward(trans.data_ptr(), pred.data_ptr(), _lab_ptr(labels),
-                                                  label_lens.data_ptr(), act_lens.data_ptr(), V, N,
-                                                  costs.data_ptr(), 1 if need else 0, ws.data_ptr(),
-                                                  _joint_opts(trans, pred, blank))
-        if st != 0:
-            raise RuntimeError("rnnt_b200_add_joint_forward failed: " + warp_rnnt.status_string(st))
+            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, need, blank, smooth)
         length_check.finish()   # the reference's length test, waited for with the kernels already queued
         if need:
             ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
-            ctx.ws, ctx.blank, ctx.gopt = ws, blank, gopt
+            ctx.ws, ctx.blank, ctx.gopt, ctx.smooth = ws, blank, gopt, smooth
             ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -146,13 +206,16 @@ class _AddJointRNNT(Function):
             args = (trans.data_ptr(), pred.data_ptr(), dtrans.data_ptr(), dpred.data_ptr(), _lab_ptr(labels),
                     label_lens.data_ptr(), act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale)
             tail = (ctx.ws.data_ptr(), _joint_opts(trans, pred, ctx.blank))
-            if ctx.gopt is not None:
+            if ctx.smooth is not None:
+                gopt = warp_rnnt.rnntGradOptions() if ctx.gopt is None else ctx.gopt
+                st = _lib.rnnt_b200_add_joint_smoothed_backward(*args, gopt, ctx.smooth, *tail)
+            elif ctx.gopt is not None:
                 st = _lib.rnnt_b200_add_joint_backward_ex(*args, ctx.gopt, *tail)
             else:
                 st = _lib.rnnt_b200_add_joint_backward(*args, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_add_joint_backward failed: " + warp_rnnt.status_string(st))
-        return dtrans, dpred, None, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None, None, None
 
 
 def _no_clamp(clamp):
@@ -162,19 +225,24 @@ def _no_clamp(clamp):
 
 
 def add_joint_rnnt_loss(trans, pred, labels, act_lens, label_lens, blank=0, reduction='mean', *,
-                        fastemit_lambda=0.0, clamp=None):
-    """fastemit_lambda: as rnnt_loss (the gradient is then not the gradient of the returned loss)."""
+                        fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0, am_only_scale=0.0):
+    """fastemit_lambda: as rnnt_loss (the gradient is then not the gradient of the returned loss).
+    lm_only_scale, am_only_scale: the smoothed loss (module docstring); both 0 is the plain loss."""
     _no_clamp(clamp)
-    return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda)
+    return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
+                               lm_only_scale, am_only_scale)
 
 
 class AddJointRNNTLoss(Module):
-    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=None):
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0,
+                 am_only_scale=0.0):
         super().__init__()
         _no_clamp(clamp)
         warp_rnnt.grad_options(fastemit_lambda)
+        smooth_options(lm_only_scale, am_only_scale)
         self.blank, self.reduction, self.fastemit_lambda = blank, reduction, fastemit_lambda
+        self.lm_only_scale, self.am_only_scale = lm_only_scale, am_only_scale
 
     def forward(self, trans, pred, labels, act_lens, label_lens):
         return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, self.blank, self.reduction,
-                                   self.fastemit_lambda)
+                                   self.fastemit_lambda, self.lm_only_scale, self.am_only_scale)

@@ -20,7 +20,7 @@ from torch.nn import Module
 
 from . import warp_rnnt
 from ._checks import LengthCheck, check_contiguous, check_dim, check_type
-from .joint import _AddJointRNNT, _joint_opts, _lab_ptr, certify_joint_inputs
+from .joint import _AddJointRNNT, _joint_opts, _lab_ptr, check_joint_call, joint_forward_call
 
 _lib = warp_rnnt.lib()
 _P = C.c_void_p
@@ -55,42 +55,28 @@ class _AddJointRNNTRanges(Function):
     """_AddJointRNNT's forward with beta always kept, plus the ranges kernel on its workspace; the same backward."""
 
     @staticmethod
-    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, s_range):
-        gopt = warp_rnnt.grad_options(fastemit_lambda)   # ValueError before any device work
-        if gopt is not None:
-            gopt.clamp = 0.0
+    def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, s_range,
+                lm_only_scale=0.0, am_only_scale=0.0):
         s_range = int(s_range)
         if s_range < 2:
             raise ValueError("s_range must be >= 2, got %d" % s_range)
-        length_check = certify_joint_inputs(trans, pred, labels, act_lens, label_lens, defer=True)
-        if not trans.is_cuda:
-            raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only")
-        warp_rnnt.require_same_device(trans, pred=pred, labels=labels, act_lens=act_lens, label_lens=label_lens)
-        if reduction not in ('none', 'sum', 'mean'):
-            raise ValueError("reduction must be 'none', 'sum' or 'mean'")
-        N, T, V = trans.shape
-        U = pred.shape[1]
+        gopt, smooth, length_check = check_joint_call(trans, pred, labels, act_lens, label_lens, reduction,
+                                                      fastemit_lambda, lm_only_scale, am_only_scale)
+        N, T = trans.shape[0], trans.shape[1]
         length_check.guard_labels(labels, N)
         costs = torch.empty(N, dtype=torch.float32, device=trans.device)
         ranges = torch.empty((N, T), dtype=torch.int32, device=trans.device)
-        n = C.c_size_t(0)
-        _lib.rnnt_b200_add_joint_workspace_size(T, U, N, V, C.byref(n))
         with torch.cuda.device(trans.device):
-            ws = torch.empty(n.value, dtype=torch.uint8, device=trans.device)
-            opts = _joint_opts(trans, pred, blank)
-            st = _lib.rnnt_b200_add_joint_forward(trans.data_ptr(), pred.data_ptr(), _lab_ptr(labels),
-                                                  label_lens.data_ptr(), act_lens.data_ptr(), V, N,
-                                                  costs.data_ptr(), 1, ws.data_ptr(), opts)
-            if st != 0:
-                raise RuntimeError("rnnt_b200_add_joint_forward failed: " + warp_rnnt.status_string(st))
+            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, True, blank, smooth)
             st = _lib.rnnt_b200_add_joint_prune_ranges(label_lens.data_ptr(), act_lens.data_ptr(), N, s_range,
-                                                       ranges.data_ptr(), ws.data_ptr(), opts)
+                                                       ranges.data_ptr(), ws.data_ptr(),
+                                                       _joint_opts(trans, pred, blank))
         if st != 0:
             raise RuntimeError("rnnt_b200_add_joint_prune_ranges failed: " + warp_rnnt.status_string(st))
         length_check.finish()
         ctx.mark_non_differentiable(ranges)
         ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
-        ctx.ws, ctx.blank, ctx.gopt = ws, blank, gopt
+        ctx.ws, ctx.blank, ctx.gopt, ctx.smooth = ws, blank, gopt, smooth
         ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -101,16 +87,18 @@ class _AddJointRNNTRanges(Function):
     @staticmethod
     def backward(ctx, grad_output, grad_ranges):
         dtrans, dpred = _AddJointRNNT.backward(ctx, grad_output)[:2]
-        return dtrans, dpred, None, None, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None, None, None, None
 
 
 def add_joint_rnnt_loss_with_ranges(trans, pred, labels, act_lens, label_lens, s_range, blank=0, reduction='mean',
-                                    *, fastemit_lambda=0.0):
+                                    *, fastemit_lambda=0.0, lm_only_scale=0.0, am_only_scale=0.0):
     """(loss, ranges): add_joint_rnnt_loss (the "simple" loss of pruned RNN-T; differentiable in trans and pred
     exactly as add_joint_rnnt_loss) and the [N, T] int32 window starts of the pruned loss for R = s_range >= 2,
-    from the same forward (include/rnnt.h, rnnt_b200_add_joint_prune_ranges, defines them)."""
+    from the same forward (include/rnnt.h, rnnt_b200_add_joint_prune_ranges, defines them).  lm_only_scale and
+    am_only_scale smooth the simple loss as add_joint_rnnt_loss's do (icefall's --lm-scale / --am-scale); the
+    windows then come from the smoothed lattice."""
     return _AddJointRNNTRanges.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
-                                     s_range)
+                                     s_range, lm_only_scale, am_only_scale)
 
 
 def prune_joint_inputs(enc, dec, ranges, s_range):
