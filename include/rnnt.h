@@ -278,6 +278,8 @@ rnntStatus_t rnnt_b200_backward_ex(int dtype, const void* activations, void* gra
  * grad_trans = grad_scale * d cost/d trans, grad_pred likewise (docs/rnnt_notes.tex:147-153).
  * All pointers DEVICE, fp32, no synchronisation.  Workspace from rnnt_b200_add_joint_workspace_size.
  * HBM traffic is O(N (T+U) V) instead of O(N T U V).
+ * Padded rows (trans frames t >= input_lengths[b], pred rows u > label_lengths[b]) are not read, so they may hold
+ * anything, NaN and inf included, and get a zero gradient.
  */
 rnntStatus_t rnnt_b200_add_joint_loss(const float* trans, const float* pred, float* grad_trans,
                                       float* grad_pred, const int* flat_labels,
@@ -316,7 +318,8 @@ rnntStatus_t rnnt_b200_add_joint_backward_ex(const float* trans, const float* pr
  *   La(t) = log sum_v exp(f[t,v]) ug[v]                    the am-only normaliser
  * The gradients are the exact gradients of the returned cost in trans and pred, including the path through ug: with
  * am_only_scale > 0 one utterance's grad_pred depends on the whole batch.  FastEmit scales the gradient of each
- * (interpolated) label factor by 1 + fastemit_lambda.  Padded rows of pred are not read and get a zero gradient.
+ * (interpolated) label factor by 1 + fastemit_lambda.  Padded rows of trans and pred are not read (they may hold NaN
+ * or inf) and get a zero gradient, as in the plain joint.
  * Valid scales are finite, >= 0, with lm_only_scale + am_only_scale <= 1 + 2^-23 (one float32 ulp of slack, so
  * that pairs meant to sum to 1, such as (0.6f, 0.4f), are accepted; c is then 0); anything else returns
  * RNNT_STATUS_INVALID_VALUE before any device access.  Both scales 0 is the plain joint, bitwise.

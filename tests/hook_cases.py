@@ -1,7 +1,10 @@
 """Child process of test_gpu_tuning_hooks.py: runs one suite of shapes through the library with the tuning hooks
 (RNNT_B200_* environment variables, README) already set in its environment, and checks each against the fp64 oracle.
 
-    python tests/hook_cases.py {dense|joint} OUT_DIR
+    python tests/hook_cases.py {dense|joint|smoothed} OUT_DIR
+
+"smoothed" runs the JOINT shapes with lm_only_scale 0.25 and am_only_scale 0.1 (DESIGN.md §9) and checks them
+against the closed-form fp64 reference (tests/smoothed_reference.py).
 
 A hook is read once per process into a static, so every hook setting needs a process of its own.  Saves each
 shape's costs and gradients to OUT_DIR/<shape>.npz and prints one JSON line:
@@ -24,8 +27,10 @@ for p in (ROOT, os.path.join(ROOT, "warp-transducer_b200"), os.path.dirname(os.p
 import torch  # noqa: E402
 from torch.profiler import ProfilerActivity, profile  # noqa: E402
 
+import smoothed_reference  # noqa: E402
 from joint_reference import grad_mismatch, reference as joint_reference  # noqa: E402
 from oracle import pyoracle  # noqa: E402
+from test_gpu_add_joint_smoothed import FLOOR_DENSE_AM  # noqa: E402
 
 # (N, T, U, V): N = 10 >= 8 so that RNNT_B200_GROUPS applies (uneven groups for 3 and 8); full calls with gradients
 DENSE = {
@@ -43,6 +48,11 @@ JOINT = {
     "U40_V1000": (2, 24, 40, 1000),      # two-kernel gradient, 3 split-K slabs / joint_thin_kernel
     "U8_V5121": (2, 16, 8, 5121),        # 16 split-K slabs, the last empty
 }
+SMOOTH = (0.25, 0.1)   # (lm_only_scale, am_only_scale) of the smoothed suite
+# dG's dense-column floor of the smoothed suite (joint_reference's default, FLOOR_DENSE_AM for am_only_scale > 0), and
+# per shape where a hook needs more.  U8_V5121: RNNT_B200_JOINT_SLICES=1 sums all 5121 columns of S in one
+# tensor-core accumulation instead of 16 slabs; measured 1.79e-7 on an H100 80GB HBM3 at 700 W.
+SMOOTH_FLOOR_DENSE = {"U8_V5121": 3e-7}
 
 
 def inputs(name, shape, joint):
@@ -89,6 +99,30 @@ def run_joint(wr, trans, pred, labels, tl, ul):
     return costs.cpu().numpy(), dF.cpu().numpy(), dG.cpu().numpy(), launches
 
 
+def run_smoothed(wr, trans, pred, labels, tl, ul):
+    from warprnnt_pytorch.joint import add_joint_rnnt_loss
+    tt = torch.tensor(trans, device="cuda", requires_grad=True)
+    pp = torch.tensor(pred, device="cuda", requires_grad=True)
+    lab, tld, uld = (torch.as_tensor(x).cuda() for x in (labels, tl, ul))
+    out = add_joint_rnnt_loss(tt, pp, lab, tld, uld, 0, 'none', lm_only_scale=SMOOTH[0], am_only_scale=SMOOTH[1])
+    out.sum().backward()
+    launches = wr.last_launch_count()
+    torch.cuda.synchronize()
+    return out.detach().cpu().numpy(), tt.grad.cpu().numpy(), pp.grad.cpu().numpy(), launches
+
+
+def check_smoothed(name, out, x, labels, tl, ul):
+    costs, dF, dG = out
+    c_ref, dF_ref, dG_ref = smoothed_reference.closed_form(x[0], x[1], labels, tl, ul, *SMOOTH)
+    problems = []
+    if not np.allclose(costs, c_ref, rtol=1e-5, atol=1e-5):
+        problems.append("costs: max |err| %.3g" % np.abs(costs - c_ref).max())
+    floor = SMOOTH_FLOOR_DENSE.get(name, FLOOR_DENSE_AM)
+    problems += grad_mismatch(dF, dF_ref, tl, labels, ul, 0, "dF", floor_dense=floor)
+    problems += grad_mismatch(dG, dG_ref, ul + 1, labels, ul, 0, "dG", floor_dense=floor)
+    return problems
+
+
 def check_dense(out, acts, labels, tl, ul):
     costs, grads = out
     c_ref, g_ref, _ = pyoracle.rnnt_logits(acts.astype(np.float64), labels, tl, ul, 0)
@@ -117,18 +151,19 @@ def main():
     lib = wr.lib()
     lib.rnnt_b200_debug_policy.restype = C.c_int
     lib.rnnt_b200_debug_policy.argtypes = [C.c_int, C.c_int, C.c_int]
-    joint = suite == "joint"
+    joint = suite in ("joint", "smoothed")
     shapes = JOINT if joint else DENSE
+    run = {"dense": run_dense, "joint": run_joint, "smoothed": run_smoothed}[suite]
     results, kernels = {}, set()
     for name, shape in shapes.items():
         x, labels, tl, ul = inputs(name, shape, joint)
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            if joint:
-                *out, launches = run_joint(wr, x[0], x[1], labels, tl, ul)
-            else:
-                *out, launches = run_dense(wr, x, labels, tl, ul)
+            *out, launches = run(wr, *(x if joint else (x,)), labels, tl, ul)
         kernels.update(e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
-        problems = check_joint(out, x, labels, tl, ul) if joint else check_dense(out, x, labels, tl, ul)
+        if suite == "smoothed":
+            problems = check_smoothed(name, out, x, labels, tl, ul)
+        else:
+            problems = (check_joint if joint else check_dense)(out, x, labels, tl, ul)
         keys = ("costs", "dF", "dG") if joint else ("costs", "grads")
         np.savez(os.path.join(out_dir, name + ".npz"), **dict(zip(keys, out)))
         results[name] = {"ok": not problems, "problems": problems, "launches": launches}

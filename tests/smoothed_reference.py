@@ -11,7 +11,9 @@ With f = trans [N,T,V], g = pred [N,U,V], U_b = label_len_b + 1 and c = 1 - lm -
 A term whose scale is exactly 0 is left out.  The cost is -log-likelihood of the standard lattice on these factors
 (pruned_reference.lattice).  factors() / costs() are numpy; torch_costs() is the same forward in torch fp64, whose
 autograd is the reference gradient (it includes the path through ug).  smoothed_occupancies() feeds
-pruned_reference.prune_ranges the windows of the smoothed lattice.
+pruned_reference.prune_ranges the windows of the smoothed lattice.  closed_form() gives reference()'s results from
+the chain rule written out term by term, one utterance at a time: it never forms [T, U, V] and reaches training
+shapes that the autograd reference cannot.
 """
 import numpy as np
 
@@ -163,3 +165,101 @@ def reference(trans, pred, labels, act_lens, label_lens, lm=0.0, am=0.0, blank=0
     (c * w).sum().backward()
     grad = lambda x: np.zeros(x.shape) if x.grad is None else x.grad.numpy()   # noqa: E731  (lm = 1: no trans path)
     return c.detach().numpy(), grad(f), grad(g)
+
+
+# ---- closed form: the same costs and gradients without autograd and without any [T, U, V] array ------------------
+def _exp_rows(x):
+    """(E = exp(x - m), m) per row, m the row max (0 for an all -inf row)."""
+    m = x.max(axis=1)
+    m = np.where(np.isfinite(m), m, 0.0)
+    return np.exp(x - m[:, None]), m
+
+
+def closed_form(trans, pred, labels, act_lens, label_lens, lm=0.0, am=0.0, blank=0, fastemit_lambda=0.0, scale=None):
+    """reference()'s (costs [N], dF [N,T,V], dG [N,U,V]) in float64, from the factor formula and the chain rule.
+
+    Per utterance, with Ef = exp(f - mf), Eg = exp(g - mg), S = Ef Eg^T, sg = rowsum Eg, A = Ef ug, the occupancies
+    of the smoothed lattice Bk (blank) and Lb = (1 + lambda) e_y (label), both times scale[b], and O = Bk + Lb:
+      full term (c):   dF = c (Ef * ((O/S) Eg) - sparse_f),      dG = c (Eg * ((O/S)^T Ef) - sparse_g)
+      lm-only term:    dG += lml (O_u Eg / sg - sparse_g)           O_u = sum_t O
+      am-only term:    dF += lma (O_t Ef ug / A - sparse_f)         O_t = sum_u O
+      through ug:      h[v] = lma (sum_{b,t} O_t Ef[t,v] / A(t) - Z[v] / ug[v]),  dG += Eg / (M sg) (h - hbar_u)
+    sparse_f / sparse_g put Bk on the blank column and Lb on the label columns; Z[v] sums them over the batch,
+    hbar_u = sum_v Eg[u,v] h[v] / sg(u).  One utterance at a time, plus one batch vector for h."""
+    N, T, V = trans.shape
+    U = pred.shape[1]
+    c = 1.0 - lm - am
+    labels = np.asarray(labels)
+    s = np.ones(N) if scale is None else np.asarray(scale, np.float64)
+    ext = extents(act_lens, label_lens, T, U)
+    preds = []   # (g, Eg, mg, sg) of the valid rows
+    for b, (_, Ub) in enumerate(ext):
+        g = np.asarray(pred[b, :Ub], np.float64)
+        Eg, mg = _exp_rows(g)
+        preds.append((g, Eg, mg, Eg.sum(axis=1)))
+    M = sum(Ub for _, Ub in ext)
+    if am != 0.0:
+        ug = sum((Eg / sg[:, None]).sum(axis=0) for _, Eg, _, sg in preds) / M + FLT_MIN
+        hsum, Z = np.zeros(V), np.zeros(V)
+    costs, dF, dG = np.zeros(N), np.zeros((N, T, V)), np.zeros((N, U, V))
+    for b, (Tb, Ub) in enumerate(ext):
+        g, Eg, mg, sg = preds[b]
+        f = np.asarray(trans[b, :Tb], np.float64)
+        Ef, mf = _exp_rows(f)
+        S = Ef @ Eg.T
+        lse = mf[:, None] + mg[None, :] + np.log(S)
+        Lg = mg + np.log(sg)
+        if am != 0.0:
+            A = Ef @ ug
+            La = mf + np.log(A)
+        y = labels[b, :Ub - 1].astype(np.int64) if Ub > 1 else np.zeros(0, np.int64)
+
+        def lp(k):
+            n = len(k)
+            fk, gk = f[:, k], g[np.arange(n), k][None, :]
+            out = np.zeros((Tb, n))
+            if c != 0.0:
+                out += c * (fk + gk - lse[:, :n])
+            if lm != 0.0:
+                out += lm * (gk - Lg[None, :n])
+            if am != 0.0:
+                out += am * (fk + np.log(ug[k])[None, :] - La[:, None])
+            return out
+
+        lpb, lpy = lp(np.full(Ub, blank, np.int64)), lp(y)
+        alpha, beta, ll = lattice(lpb, lpy)
+        costs[b] = -ll
+        beta_next = np.full((Tb, Ub), -np.inf)   # beta(t+1, u), with the final blank into beta(T_b, U_b-1) = 0
+        beta_next[:Tb - 1] = beta[1:]
+        beta_next[Tb - 1, Ub - 1] = 0.0
+        Bk = s[b] * np.exp(alpha + lpb + beta_next - ll)
+        Lb = s[b] * (1.0 + fastemit_lambda) * np.exp(alpha[:, :Ub - 1] + lpy + beta[:, 1:] - ll)
+        O = Bk.copy()
+        O[:, :Ub - 1] += Lb
+        sp_f, sp_g = np.zeros((Tb, V)), np.zeros((Ub, V))
+        sp_f[:, blank] += Bk.sum(axis=1)
+        sp_g[:, blank] += Bk.sum(axis=0)
+        for u in range(Ub - 1):
+            sp_f[:, y[u]] += Lb[:, u]
+            sp_g[u, y[u]] += Lb[:, u].sum()
+        dFb, dGb = -(c + am) * sp_f, -(c + lm) * sp_g
+        if c != 0.0:
+            W = O / S
+            dFb += c * Ef * (W @ Eg)
+            dGb += c * Eg * (W.T @ Ef)
+        if lm != 0.0:
+            dGb += lm * (O.sum(axis=0) / sg)[:, None] * Eg
+        if am != 0.0:
+            wt = O.sum(axis=1) / A   # O_t / A(t)
+            dFb += am * wt[:, None] * Ef * ug[None, :]
+            hsum += wt @ Ef
+            Z[blank] += Bk.sum()
+            np.add.at(Z, y, Lb.sum(axis=0))
+        dF[b, :Tb], dG[b, :Ub] = dFb, dGb
+    if am != 0.0:
+        h = am * (hsum - Z / ug)
+        for b, (_, Ub) in enumerate(ext):
+            _, Eg, _, sg = preds[b]
+            R = Eg / sg[:, None]
+            dG[b, :Ub] += R * (h[None, :] - (R @ h)[:, None]) / M
+    return costs, dF, dG

@@ -1,9 +1,5 @@
 """Smoothed additive joint (lm_only_scale / am_only_scale, DESIGN.md §9) on the GPU against the fp64 reference
 (tests/smoothed_reference.py), and its identity with the plain joint at scales (0, 0)."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -13,7 +9,6 @@ from joint_reference import assert_joint_close
 from pruned_reference import prune_ranges
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 SCALES = [(0.25, 0.0), (0.0, 0.25), (0.25, 0.1), (0.5, 0.5), (1.0, 0.0), (0.0, 1.0)]
 # (N, T, U, V, blank): the dispatch each shape reaches
@@ -126,36 +121,7 @@ def test_two_calls_are_bitwise_identical(shape):
         assert np.array_equal(x, y)
 
 
-CHILD = r'''
-import os, sys, numpy as np
-sys.path[:0] = [sys.argv[1], sys.argv[2], os.path.dirname(sys.argv[1])]
-import test_gpu_add_joint_smoothed as m
-N, T, U, V, blank = m.SHAPES[sys.argv[3]]
-x = m.make_inputs(14, N, T, U, V, blank)
-out = m.run(*x, blank, 0.25, 0.1, np.linspace(0.5, 1.5, N))
-np.savez(sys.argv[4], costs=out[0], dF=out[1], dG=out[2])
-'''
-
-
-@pytest.mark.parametrize("hook,shape", [("RNNT_B200_JOINT_SIMT=1", "fused_V4k"),       # joint_thin_kernel
-                                        ("RNNT_B200_JOINT_SIMT=1", "fused_V_odd"),     # EpiGrad
-                                        ("RNNT_B200_JOINT_FUSED=0", "fused_V4k"),      # two-kernel wgmma
-                                        ("RNNT_B200_DF_TILE=128", "two_kernel_T70")])  # dF 128-column tile
-def test_tuning_hook_paths(hook, shape, tmp_path):
-    key, val = hook.split("=")
-    env = dict(os.environ, **{key: val})
-    out = str(tmp_path / "out.npz")
-    pkg = os.path.join(os.path.dirname(HERE), "warp-transducer_b200")
-    r = subprocess.run([sys.executable, "-c", CHILD, HERE, pkg, shape, out], env=env, capture_output=True, text=True,
-                       timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    got = np.load(out)
-    N, T, U, V, blank = SHAPES[shape]
-    trans, pred, labels, tl, ul = make_inputs(14, N, T, U, V, blank)
-    w = np.linspace(0.5, 1.5, N)
-    c_ref, dF_ref, dG_ref = sr.reference(trans.astype(np.float64), pred.astype(np.float64), labels, tl, ul, 0.25, 0.1,
-                                         blank, scale=w)
-    assert_joint_close(got["costs"], got["dF"], got["dG"], c_ref, dF_ref, dG_ref, labels, tl, ul, blank, **floors(0.1))
+# The tuning hooks' smoothed paths run in test_gpu_tuning_hooks.py (the "smoothed" suite of hook_cases.py).
 
 
 @pytest.mark.parametrize("lm,am", [(0.25, 0.0), (0.25, 0.1)])

@@ -34,6 +34,24 @@ CASES = {
     "JOINT_SLICES_7": ("joint", {"RNNT_B200_JOINT_SLICES": "7"}, [], [], False),
     "JOINT_SLICES_16": ("joint", {"RNNT_B200_JOINT_SLICES": "16"}, [], [], False),
     "DF_TILE_128": ("joint", {"RNNT_B200_DF_TILE": "128"}, [r"wg::gemm_kernel<3, 1, 128, 24>"], [], False),
+    # smoothed additive joint (DESIGN.md §9): each hook must run the SMOOTH instantiation of its kernels
+    "SMOOTHED_JOINT_SIMT_1": ("smoothed", {"RNNT_B200_JOINT_SIMT": "1"},
+                              [r"joint_thin_kernel<true>", r"EpiGrad<true>", r"joint_stats_kernel<true>",
+                               r"joint_gemm_kernel<b200rnnt::EpiPartial, 64, 32>"],
+                              [r"wg::gemm_kernel", r"grad_fused_kernel"], False),
+    "SMOOTHED_JOINT_FUSED_0": ("smoothed", {"RNNT_B200_JOINT_FUSED": "0"},
+                               [r"wg::gemm_kernel<3, 1, 64, 24, b200rnnt::wg::Smooth>",
+                                r"wg::gemm_kernel<0, 1, 32, 24, b200rnnt::wg::Smooth>", r"joint_stats_kernel<true>"],
+                               [r"grad_fused_kernel"], False),
+    "SMOOTHED_JOINT_SLICES_1": ("smoothed", {"RNNT_B200_JOINT_SLICES": "1"},
+                                [r"grad_fused_kernel<32, 32, 3, true>", r"joint_stats_kernel<true>"], [], False),
+    "SMOOTHED_JOINT_SLICES_7": ("smoothed", {"RNNT_B200_JOINT_SLICES": "7"},
+                                [r"grad_fused_kernel<32, 32, 3, true>", r"joint_stats_kernel<true>"], [], False),
+    "SMOOTHED_JOINT_SLICES_16": ("smoothed", {"RNNT_B200_JOINT_SLICES": "16"},
+                                 [r"grad_fused_kernel<32, 32, 3, true>", r"joint_stats_kernel<true>"], [], False),
+    "SMOOTHED_DF_TILE_128": ("smoothed", {"RNNT_B200_DF_TILE": "128"},
+                             [r"wg::gemm_kernel<3, 1, 128, 24, b200rnnt::wg::Smooth>", r"joint_stats_kernel<true>"],
+                             [], False),
     # dense loss
     "CHUNK_0": ("dense", {"RNNT_B200_CHUNK": "0"}, [r"grad_tile_kernel<float, 4, 2,", r"grad_tile_kernel<float, 2, 4,"],
                 [r"grad_chunk_kernel", r"rowstats_chunk_kernel"], False),
@@ -88,7 +106,7 @@ def run_child(suite, env_extra, out_dir):
 def baseline(tmp_path_factory):
     """The default dispatch, one child per suite (no hook set)."""
     out = {}
-    for suite in ("dense", "joint"):
+    for suite in ("dense", "joint", "smoothed"):
         d = str(tmp_path_factory.mktemp("baseline_" + suite))
         out[suite] = (run_child(suite, {}, d), d)
     return out
@@ -102,6 +120,7 @@ def test_default_dispatch_matches_the_oracle(baseline):
     assert dense["policy"]["pdl"] == 0
     assert all(res["launches"] == 3 for res in dense["shapes"].values())
     assert any("grad_fused_kernel" in k for k in baseline["joint"][0]["kernels"])
+    assert any("grad_fused_kernel<32, 32, 3, true>" in k for k in baseline["smoothed"][0]["kernels"])
 
 
 @pytest.mark.parametrize("case", list(CASES))

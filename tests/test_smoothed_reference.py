@@ -102,6 +102,77 @@ def test_padded_pred_rows_are_not_read(lm, am):
         assert not dG[b, int(ul[b]) + 1:].any() and not dF[b, int(tl[b]):].any()
 
 
+def assert_rel_close(got, want, rtol=1e-10):
+    """Elementwise within rtol of the array's largest magnitude (the gradients hold exact zeros and tiny values)."""
+    for g, w in zip(got, want):
+        assert g.shape == w.shape
+        assert np.abs(g - w).max() <= rtol * max(np.abs(w).max(), 1e-300), np.abs(g - w).max() / np.abs(w).max()
+
+
+def assert_closed_form_matches(x, lm, am, **kw):
+    trans, pred, labels, tl, ul = x
+    got = sr.closed_form(trans, pred, labels, tl, ul, lm, am, **kw)
+    want = sr.reference(trans, pred, labels, tl, ul, lm, am, **kw)
+    assert_rel_close(got, want)
+    return got
+
+
+@pytest.mark.parametrize("lm,am", SCALES + [(0.0, 0.0), (0.6, 0.4)])   # c = 0 at (1, 0), (0, 1) and (0.6, 0.4)
+def test_closed_form_equals_autograd(lm, am):
+    got = assert_closed_form_matches(problem(20, N=3, T=6, U=5, V=9), lm, am)
+    if lm == 1.0:
+        assert not got[1].any()
+
+
+@pytest.mark.parametrize("lm,am", [(0.25, 0.0), (0.25, 0.1), (0.0, 1.0)])
+def test_closed_form_fastemit_and_signed_scale(lm, am):
+    x = problem(21, N=3, T=5, U=4, V=8)
+    assert_closed_form_matches(x, lm, am, fastemit_lambda=0.3, scale=np.array([0.5, -1.25, 2.0]))
+
+
+@pytest.mark.parametrize("lm,am", [(0.25, 0.1), (0.5, 0.5)])
+def test_closed_form_edges(lm, am):
+    # one frame per utterance; blank = V - 1
+    trans, pred, labels, _, ul = problem(22, N=3, T=4, U=4, V=6)
+    labels = np.minimum(labels, 4).astype(np.int32)   # labels in 1..4, never the blank 5
+    assert_closed_form_matches((trans, pred, labels, np.ones(3, np.int32), ul), lm, am, blank=5)
+    # every U_b = 1: no labels, ug over N pred rows
+    trans, pred, labels, tl, _ = problem(23, N=3, T=5, U=3, V=7)
+    assert_closed_form_matches((trans, pred, labels, tl, np.zeros(3, np.int32)), lm, am)
+
+
+@pytest.mark.parametrize("lm,am", [(0.25, 0.1), (0.0, 0.25), (0.0, 0.0)])
+def test_closed_form_masked_vocabulary_columns(lm, am):
+    trans, pred, labels, tl, ul = problem(24, N=3, T=5, U=4, V=10)
+    labels = np.where(labels >= 7, labels - 6, labels).astype(np.int32)   # columns 7..9 are neither blank nor label
+    trans[:, :, 7:] = -np.inf
+    c, dF, dG = assert_closed_form_matches((trans, pred, labels, tl, ul), lm, am)
+    assert np.all(np.isfinite(c)) and not dF[:, :, 7:].any()
+
+
+def test_closed_form_zero_scales_equal_the_joint_reference():
+    from joint_reference import reference
+    trans, pred, labels, tl, ul = problem(25, N=3, T=6, U=5, V=8)
+    f32 = lambda x: x.astype(np.float32).astype(np.float64)   # noqa: E731  the oracle saw float32 inputs
+    c_ref, dF_ref, dG_ref = reference(trans.astype(np.float32), pred.astype(np.float32), labels, tl, ul, 0)
+    assert_rel_close(sr.closed_form(f32(trans), f32(pred), labels, tl, ul), (c_ref, dF_ref, dG_ref))
+
+
+def test_closed_form_reaches_the_training_shape_in_bounded_memory():
+    """One C3-sized utterance (T 150, U 21, V 5000): the closed form holds O((T + U) V) per utterance."""
+    rng = np.random.default_rng(26)
+    N, T, U, V = 2, 150, 21, 5000
+    trans = rng.standard_normal((N, T, V)).astype(np.float32)
+    pred = rng.standard_normal((N, U, V)).astype(np.float32)
+    labels = rng.integers(1, V, size=(N, U - 1)).astype(np.int32)
+    tl, ul = np.array([T, 97], np.int32), np.array([U - 1, 13], np.int32)
+    c, dF, dG = sr.closed_form(trans, pred, labels, tl, ul, 0.25, 0.1)
+    assert np.all(np.isfinite(c)) and np.isfinite(dF).all() and np.isfinite(dG).all()
+    assert np.allclose(c, sr.costs(trans, pred, labels, tl, ul, 0.25, 0.1), rtol=1e-12)
+    # every logit's gradient sums to 0 over v, and the am-only / lm-only / full terms each do: so do dF and dG rows
+    assert np.abs(dF.sum(-1)).max() < 1e-9 and np.abs(dG.sum(-1)).max() < 1e-9
+
+
 # ---- argument rules of the smoothed entries (host buffers, rejected before any device access) ----------------------
 @pytest.fixture(scope="module")
 def abi():

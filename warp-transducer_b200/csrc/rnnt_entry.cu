@@ -981,36 +981,38 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
     const bool with_beta = dF != nullptr || c.want_beta;
 
     if (c.phase != kBackward) {
-    // J1: factor-wise max and exponentials (SUM: and sum[row] = sum_k e_k wv[k], wv NULL: 1)
-    auto prep = [&](auto sum, const float* x, float* e, float* mx, int rows, const float* wv = nullptr,
-                    float* rowsum = nullptr) {
+    // J1: factor-wise max and exponentials (SUM: and sum[row] = sum_k e_k wv[k], wv NULL: 1); padded rows (t >= T_b
+    // of f, u >= U_b of g) are not read and come out as zeros
+    auto prep = [&](auto sum, const float* x, float* e, float* mx, const int* len, int add, int R,
+                    const float* wv = nullptr, float* rowsum = nullptr) {
         constexpr bool SUM = decltype(sum)::value;
+        const int rows = N * R;
         const int per = (V / 4 + 255) / 256;   // float4 per thread when one CTA owns a row
         const bool vec = V % 4 == 0 && per <= 8 && V >= 1024 && reinterpret_cast<uintptr_t>(x) % 16 == 0;
-        if (!vec) joint_prep_kernel<SUM><<<(rows + 7) / 8, 256, 0, s>>>(x, e, mx, rows, V, wv, rowsum);
-        else if (per <= 1) joint_prep_row_kernel<1, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
-        else if (per <= 2) joint_prep_row_kernel<2, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
-        else if (per <= 4) joint_prep_row_kernel<4, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
-        else if (per <= 5) joint_prep_row_kernel<5, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
-        else joint_prep_row_kernel<8, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, wv, rowsum);
+        if (!vec) joint_prep_kernel<SUM><<<(rows + 7) / 8, 256, 0, s>>>(x, e, mx, rows, V, len, add, R, wv, rowsum);
+        else if (per <= 1) joint_prep_row_kernel<1, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, len, add, R, wv, rowsum);
+        else if (per <= 2) joint_prep_row_kernel<2, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, len, add, R, wv, rowsum);
+        else if (per <= 4) joint_prep_row_kernel<4, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, len, add, R, wv, rowsum);
+        else if (per <= 5) joint_prep_row_kernel<5, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, len, add, R, wv, rowsum);
+        else joint_prep_row_kernel<8, SUM><<<rows, 256, 0, s>>>(x, e, mx, V, len, add, R, wv, rowsum);
     };
     using Plain = std::false_type;
     using Sum = std::true_type;
     if (!sm) {
-        prep(Plain{}, f, w.ef, w.mf, N * T);
-        prep(Plain{}, g, w.eg, w.mg, N * U);
+        prep(Plain{}, f, w.ef, w.mf, xlen, 0, T);
+        prep(Plain{}, g, w.eg, w.mg, ylen, 1, U);
     } else {
         // g first (Eg and its row sums sg), then the unigram of the valid pred rows, then f (with A = Ef . ug)
-        prep(Sum{}, g, w.eg, w.mg, N * U, nullptr, w.sg);
+        prep(Sum{}, g, w.eg, w.mg, ylen, 1, U, nullptr, w.sg);
         if (lma != 0.0f) {
             const int chunks = smooth_chunks(N * U);
             joint_colsum_kernel<true><<<dim3((V + 255) / 256, chunks), 256, 0, s>>>(w.eg, w.sg, ylen, 1, N, U, V,
                                                                                   chunks, w.cpart);
             joint_unigram_kernel<<<(V + 255) / 256, 256, 0, s>>>(w.cpart, chunks, ylen, N, U, V, w.ug, w.lug, w.msum);
-            prep(Sum{}, f, w.ef, w.mf, N * T, w.ug, w.A);
+            prep(Sum{}, f, w.ef, w.mf, xlen, 0, T, w.ug, w.A);
             g_last_launches += 2;
         } else {
-            prep(Plain{}, f, w.ef, w.mf, N * T);
+            prep(Plain{}, f, w.ef, w.mf, xlen, 0, T);
         }
     }
     // J2: S = Ef . Eg^T in kJointSlices deterministic K-slabs, then lse + lattice log-prob pairs

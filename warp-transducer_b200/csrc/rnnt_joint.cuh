@@ -29,15 +29,32 @@ struct JointDims {
 };
 
 // ---- J1: per row of a factor: max and exp(x - max) ------------------------------------------------
+// Rows come R per utterance (R = T for f, U for g); row r of utterance b is valid iff r < clamp(len[b] + add, 1, R)
+// (len = xlen, add = 0 for f; len = ylen, add = 1 for g).  A padded row is never read: its exponentials, max and
+// sum are written as 0, so whatever the caller left there (NaN, inf) cannot reach a contraction as 0 * NaN.
+__device__ __forceinline__ bool joint_row_valid(const int* __restrict__ len, int add, int R, int row) {
+    const int b = row / R;
+    return row - b * R < min(max(__ldg(len + b) + add, 1), R);
+}
+
 // one warp per row of V elements (rows = N*T for f, N*U for g)
 // SUM (smoothing, DESIGN.md §9): also sum[row] = sum_k e_k * wv[k] (wv NULL: 1) from the exponentials in registers
 template <bool SUM = false>
 __global__ void __launch_bounds__(256)
 joint_prep_kernel(const float* __restrict__ x, float* __restrict__ e, float* __restrict__ mx, int rows, int V,
-                  const float* __restrict__ wv, float* __restrict__ sum) {
+                  const int* __restrict__ len, int add, int R, const float* __restrict__ wv, float* __restrict__ sum) {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= rows) return;
+    if (!joint_row_valid(len, add, R, row)) {
+        float* q = e + (size_t)row * V;
+        for (int k = lane; k < V; k += 32) q[k] = 0.0f;
+        if (lane == 0) {
+            mx[row] = 0.0f;
+            if (SUM) sum[row] = 0.0f;
+        }
+        return;
+    }
     const float* p = x + (size_t)row * V;
     float m = -INFINITY;
     for (int k = lane; k < V; k += 32) m = fmaxf(m, __ldg(p + k));
@@ -65,9 +82,19 @@ joint_prep_kernel(const float* __restrict__ x, float* __restrict__ e, float* __r
 template <int NV, bool SUM = false>
 __global__ void __launch_bounds__(256)
 joint_prep_row_kernel(const float* __restrict__ x, float* __restrict__ e, float* __restrict__ mx, int V,
-                      const float* __restrict__ wv, float* __restrict__ sum) {
+                      const int* __restrict__ len, int add, int R, const float* __restrict__ wv,
+                      float* __restrict__ sum) {
     __shared__ float sh[8];
     const int row = blockIdx.x, nv = V >> 2;
+    if (!joint_row_valid(len, add, R, row)) {   // the whole CTA takes this branch
+        float4* q = reinterpret_cast<float4*>(e + (size_t)row * V);
+        for (int i = threadIdx.x; i < nv; i += 256) q[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (threadIdx.x == 0) {
+            mx[row] = 0.0f;
+            if (SUM) sum[row] = 0.0f;
+        }
+        return;
+    }
     const float4* p = reinterpret_cast<const float4*>(x + (size_t)row * V);
     float4 v[NV];
 #pragma unroll
