@@ -111,11 +111,11 @@ __device__ __forceinline__ void chunk_issue(const T* __restrict__ acts, T* tile,
 // The CTA size NT is a template parameter (tuning hook RNNT_B200_CHUNK_NT; default 256).
 // =================================================================================================
 template <typename T, int TPR, int NT, bool PRUNED>
-__device__ __forceinline__ void rowstats_chunk(const T* __restrict__ acts, const int* __restrict__ labels,
-                                               const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                               typename Real<T>::pair* __restrict__ stat,
-                                               typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor,
-                                               const uint32_t wait_ns, const Prune* p) {
+__global__ void __launch_bounds__(NT)
+rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels, const int* __restrict__ xlen,
+                      const int* __restrict__ ylen, typename Real<T>::pair* __restrict__ stat,
+                      typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor, const uint32_t wait_ns,
+                      const Prune p) {
     using R = Real<T>;
     using Pair = typename R::pair;
     constexpr int ROWS = NT / TPR;
@@ -172,8 +172,8 @@ __device__ __forceinline__ void rowstats_chunk(const T* __restrict__ acts, const
         T m = R::neg_inf();
         if (paired) {
 #pragma unroll 4
-            for (int p = h; p < (V >> 1); p += TPR) {
-                const Pair v = x2[p];
+            for (int j = h; j < (V >> 1); j += TPR) {
+                const Pair v = x2[j];
                 m = R::max(m, R::max(v.x, v.y));
             }
         } else {
@@ -185,8 +185,8 @@ __device__ __forceinline__ void rowstats_chunk(const T* __restrict__ acts, const
         T sum = 0;
         if (paired) {
 #pragma unroll 4
-            for (int p = h; p < (V >> 1); p += TPR) {
-                const Pair v = x2[p];
+            for (int j = h; j < (V >> 1); j += TPR) {
+                const Pair v = x2[j];
                 sum += es.term(v.x) + es.term(v.y);
             }
         } else {
@@ -216,53 +216,36 @@ __device__ __forceinline__ void rowstats_chunk(const T* __restrict__ acts, const
         lp2[q] = Lat<T>::make((x[d.blank] - M) - lse, y >= 0 ? (x[y] - M) - lse : T(0), y >= 0);
     }
 }
-template <typename T, int TPR, int NT>
-__global__ void __launch_bounds__(NT)
-rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels, const int* __restrict__ xlen,
-                      const int* __restrict__ ylen, typename Real<T>::pair* __restrict__ stat,
-                      typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor, const uint32_t wait_ns) {
-    rowstats_chunk<T, TPR, NT, false>(acts, labels, xlen, ylen, stat, lp2, d, hmajor, wait_ns, nullptr);
-}
-template <typename T, int TPR, int NT>
-__global__ void __launch_bounds__(NT)
-rowstats_chunk_pruned_kernel(const T* __restrict__ acts, const int* __restrict__ labels, const int* __restrict__ xlen,
-                             const int* __restrict__ ylen, typename Real<T>::pair* __restrict__ stat,
-                             typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor,
-                             const uint32_t wait_ns, const Prune p) {
-    rowstats_chunk<T, TPR, NT, true>(acts, labels, xlen, ylen, stat, lp2, d, hmajor, wait_ns, &p);
-}
 
 // =================================================================================================
 // Pass 2 on a chunk: gradient in place in shared memory, one bulk store.  Formula and per-row
 // constants as grad_row_kernel (rnnt_kernels.cuh); the blank / label corrections are applied to the
-// two affected words of the row after the sweep.  The per-row constants are fetched row-parallel (thread r
-// <-> row r: one round of loads for the whole chunk) and handed to the row's lanes through shared memory.
+// two affected words of the row after the sweep.  Each lane fetches its row's constants while the chunk is in
+// flight (fp32: one round of loads).
 // =================================================================================================
-template <typename T> struct __align__(16) ChunkRow {
+// a row's gradient constants (RowGrad), its upstream scale, and 1 / 0 / -1: valid / padding / past the tensor
+template <typename T> struct ChunkRow {
     T m, cA, cB, cL;
     T scale;
     int y;
     int valid;
-    int pad;
 };
 
 template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED>
-__device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
-                                           const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                           const typename Real<T>::pair* __restrict__ stat,
-                                           const typename Lat<T>::val* __restrict__ alphas,
-                                           const typename Lat<T>::val* __restrict__ betas,
-                                           const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                                           const T* __restrict__ scale_vec, const Dims d, const int hmajor,
-                                           const uint32_t wait_ns, const GradReg<T> reg, const Prune* p) {
+__global__ void __launch_bounds__(NT)
+grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
+                  const int* __restrict__ xlen, const int* __restrict__ ylen,
+                  const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                  const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                  const T scale_in, const T* __restrict__ scale_vec, const Dims d, const int hmajor,
+                  const uint32_t wait_ns, const GradReg<T> reg, const Prune p) {
     using R = Real<T>;
     using Pair = typename R::pair;
     constexpr int ROWS = NT / TPR;
     extern __shared__ __align__(128) unsigned char chunk_raw[];
     T* tile = reinterpret_cast<T*>(chunk_raw);
     __shared__ __align__(8) unsigned long long bar_store;
-    __shared__ ChunkRow<T> rowc[1];
-    const ChunkMap<TPR> map(hmajor);   // (ROWS entries if ROWPAR is switched on)
+    const ChunkMap<TPR> map(hmajor);
     const uint32_t bar = smem_u32(&bar_store);
     // chunks in reverse order: the tail of pass 1 is met first in L2
     const uint32_t nchunks = gridDim.x;
@@ -276,10 +259,9 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
     pdl_wait();   // (PDL) the chunk was requested ahead of the lattice kernel's completion; its output is read below
 
     // Row constants: every lane fetches its row's constants itself (lanes of a row hit the same addresses, so
-    // the loads coalesce into one request per row).  The row-parallel form (thread r <-> row r, hand-over
-    // through shared memory, as in pass 1) is kept behind ROWPAR: the extra shared-memory hop behind the barrier
-    // costs more than the saved instructions at small V, and the hand-over array costs resident CTAs per SM.
-    constexpr bool ROWPAR = false;
+    // the loads coalesce into one request per row).  Fetching them row-parallel and handing them over through
+    // shared memory, as pass 1 does, costs more than the saved instructions at small V: the extra hop sits
+    // behind the barrier, and the hand-over array costs resident CTAs per SM.
     auto fetch = [&](uint32_t row_in_chunk) {
         const bool inrange = row_in_chunk < nrows;
         const uint32_t r = r0 + (inrange ? row_in_chunk : 0);
@@ -297,10 +279,12 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
             const uint32_t ua = PRUNED ? min(u, (uint32_t)d.maxU - 1) : u;
             rg = row_grad_setup_spec(d, r, b, t, ua, xlen, ylen, labels, stat, alphas, betas, llf, Tb, Ub);
             if (SCALED && scale_vec) c.scale = __ldg(scale_vec + b) * scale_in;
-            v = inrange && !grad_padding<PRUNED>(t, u, Tb, Ub, llf, b);
+            if constexpr (PRUNED) v = inrange && !pruned_grad_padding(t, u, Tb, Ub, llf, b);
+            else v = inrange && (int)t < Tb && (int)u < Ub;
         } else {
             utt_extent(d, xlen, ylen, b, Tb, Ub);
-            v = inrange && !grad_padding<PRUNED>(t, u, Tb, Ub, llf, b);
+            if constexpr (PRUNED) v = inrange && !pruned_grad_padding(t, u, Tb, Ub, llf, b);
+            else v = inrange && (int)t < Tb && (int)u < Ub;
             rg.m = 0, rg.cA = 0, rg.cB = R::neg_inf(), rg.cL = R::neg_inf(), rg.y = -1;
             if (v) {
                 rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
@@ -312,24 +296,11 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
         }
         c.m = rg.m, c.cA = rg.cA, c.cB = rg.cB, c.cL = rg.cL, c.y = rg.y;
         c.valid = v ? 1 : (inrange ? 0 : -1);   // -1: row does not exist (past the end of the tensor)
-        c.pad = 0;
         return c;
     };
-    bool valid = false;
-    ChunkRow<T> g;
-    if constexpr (ROWPAR) {
-        static_assert(!ROWPAR, "size rowc[ROWS] before enabling");
-        if (threadIdx.x < ROWS) {
-            const ChunkRow<T> c = fetch(threadIdx.x);
-            valid = c.valid > 0;
-            rowc[threadIdx.x] = c;
-        }
-    } else {
-        g = fetch(map.row);
-        valid = g.valid > 0;
-    }
-    // one barrier: publishes the mbarrier and the row constants, and tells whether any row is a real cell
-    const bool any_valid = __syncthreads_or(valid);
+    const ChunkRow<T> g = fetch(map.row);
+    // one barrier: publishes the mbarrier, and tells whether any row is a real cell
+    const bool any_valid = __syncthreads_or(g.valid > 0);
     if (!any_valid) {   // the whole chunk is padding: zeros straight to global memory
         if (bulk) {
             constexpr int VEC = 16 / sizeof(T);
@@ -354,7 +325,6 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
     // Lanes sharing a row sit in one warp (TPR divides 32), so warp-level barriers order the reads of
     // the two special logits, the in-place sweep and the corrections.
     const int i = map.row, h = map.slice;
-    if constexpr (ROWPAR) g = rowc[i];
     const bool rvalid = g.valid > 0, inrange = g.valid >= 0;
     T* x = tile + (size_t)(inrange ? i : 0) * V;
     T xb = 0, xy = 0;
@@ -367,13 +337,13 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
     if (rvalid) {
         if ((V & 1) == 0) {   // pairs: one shared-memory load and one store per two elements
 #pragma unroll 4
-            for (int p = h; p < (V >> 1); p += TPR) {
-                Pair v = x2[p];
+            for (int j = h; j < (V >> 1); j += TPR) {
+                Pair v = x2[j];
                 v.x = R::exp2(fma(v.x - g.m, (T)R::kLog2e, g.cA));
                 v.y = R::exp2(fma(v.y - g.m, (T)R::kLog2e, g.cA));
                 if (REG) v.x = clip_grad(v.x, reg.clamp), v.y = clip_grad(v.y, reg.clamp);
                 if (SCALED) v.x *= g.scale, v.y *= g.scale;
-                x2[p] = v;
+                x2[j] = v;
             }
         } else {
 #pragma unroll 4
@@ -422,191 +392,6 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
         __syncthreads();
         for (uint32_t k = threadIdx.x; k < nelem; k += NT) gout[k] = tile[k];
     }
-}
-template <typename T, int TPR, int NT, bool SCALED, bool REG = false>
-__global__ void __launch_bounds__(NT)
-grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
-                  const int* __restrict__ xlen, const int* __restrict__ ylen,
-                  const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                  const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                  const T* __restrict__ scale_vec, const Dims d, const int hmajor, const uint32_t wait_ns,
-                  const GradReg<T> reg) {
-    using R = Real<T>;
-    using Pair = typename R::pair;
-    constexpr int ROWS = NT / TPR;
-    extern __shared__ __align__(128) unsigned char chunk_raw[];
-    T* tile = reinterpret_cast<T*>(chunk_raw);
-    __shared__ __align__(8) unsigned long long bar_store;
-    __shared__ ChunkRow<T> rowc[1];
-    const ChunkMap<TPR> map(hmajor);   // (ROWS entries if ROWPAR is switched on)
-    const uint32_t bar = smem_u32(&bar_store);
-    // chunks in reverse order: the tail of pass 1 is met first in L2
-    const uint32_t nchunks = gridDim.x;
-    const uint32_t r0 = (nchunks - 1 - blockIdx.x) * ROWS;
-    const uint32_t nrows = min((uint32_t)ROWS, d.rows - r0);
-    const int V = d.V;
-    const uint32_t nelem = nrows * (uint32_t)V;
-    const bool bulk = ((nelem * (uint32_t)sizeof(T)) & 15u) == 0;
-    if (threadIdx.x == 0 && bulk) chunk_issue<T>(acts, tile, bar, r0, nrows, V);   // the copy goes out first
-    T* gout = grads + (uint64_t)r0 * V;
-    pdl_wait();   // (PDL) the chunk was requested ahead of the lattice kernel's completion; its output is read below
-
-    // Row constants: every lane fetches its row's constants itself (lanes of a row hit the same addresses, so
-    // the loads coalesce into one request per row).  The row-parallel form (thread r <-> row r, hand-over
-    // through shared memory, as in pass 1) is kept behind ROWPAR: the extra shared-memory hop behind the barrier
-    // costs more than the saved instructions at small V, and the hand-over array costs resident CTAs per SM.
-    constexpr bool ROWPAR = false;
-    auto fetch = [&](uint32_t row_in_chunk) {
-        const bool inrange = row_in_chunk < nrows;
-        const uint32_t r = r0 + (inrange ? row_in_chunk : 0);
-        ChunkRow<T> c;
-        c.scale = scale_in;
-        uint32_t u, b, t;
-        int Tb, Ub;
-        d.decode(r, b, t, u);
-        RowGrad<T> rg;
-        bool v;
-        if constexpr (sizeof(T) == 4) {
-            // every scalar of the row is requested in ONE round of loads, validity is sorted out afterwards
-            // (addresses are in bounds for any t, u of the tensor: see the workspace slack in carve())
-            rg = row_grad_setup_spec(d, r, b, t, u, xlen, ylen, labels, stat, alphas, betas, llf, Tb, Ub);
-            if (SCALED && scale_vec) c.scale = __ldg(scale_vec + b) * scale_in;
-            v = inrange && (int)t < Tb && (int)u < Ub;
-        } else {
-            utt_extent(d, xlen, ylen, b, Tb, Ub);
-            v = inrange && (int)t < Tb && (int)u < Ub;
-            rg.m = 0, rg.cA = 0, rg.cB = R::neg_inf(), rg.cL = R::neg_inf(), rg.y = -1;
-            if (v) {
-                rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
-                if (SCALED && scale_vec) c.scale = __ldg(scale_vec + b) * scale_in;
-            }
-        }
-        if constexpr (REG) {
-            if (v) fastemit_fold(rg, reg, b, t, u, d);
-        }
-        c.m = rg.m, c.cA = rg.cA, c.cB = rg.cB, c.cL = rg.cL, c.y = rg.y;
-        c.valid = v ? 1 : (inrange ? 0 : -1);   // -1: row does not exist (past the end of the tensor)
-        c.pad = 0;
-        return c;
-    };
-    bool valid = false;
-    ChunkRow<T> g;
-    if constexpr (ROWPAR) {
-        static_assert(!ROWPAR, "size rowc[ROWS] before enabling");
-        if (threadIdx.x < ROWS) {
-            const ChunkRow<T> c = fetch(threadIdx.x);
-            valid = c.valid > 0;
-            rowc[threadIdx.x] = c;
-        }
-    } else {
-        g = fetch(map.row);
-        valid = g.valid > 0;
-    }
-    // one barrier: publishes the mbarrier and the row constants, and tells whether any row is a real cell
-    const bool any_valid = __syncthreads_or(valid);
-    if (!any_valid) {   // the whole chunk is padding: zeros straight to global memory
-        if (bulk) {
-            constexpr int VEC = 16 / sizeof(T);
-            VecT<T, VEC> z;
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) z.v[c] = 0;
-            for (uint32_t k = threadIdx.x; k < nelem / VEC; k += NT) st_stream<T, VEC>(gout + (size_t)k * VEC, z);
-            if (threadIdx.x == 0) mbar_wait(bar, 0, wait_ns);   // shared memory must outlive the in-flight copy
-        } else {
-            for (uint32_t k = threadIdx.x; k < nelem; k += NT) gout[k] = T(0);
-        }
-        return;
-    }
-    if (bulk) {
-        mbar_wait(bar, 0, wait_ns);
-    } else {
-        const T* src = acts + (uint64_t)r0 * V;
-        for (uint32_t k = threadIdx.x; k < nelem; k += NT) tile[k] = ld_scalar<T>(src + k);
-        __syncthreads();
-    }
-
-    // Lanes sharing a row sit in one warp (TPR divides 32), so warp-level barriers order the reads of
-    // the two special logits, the in-place sweep and the corrections.
-    const int i = map.row, h = map.slice;
-    if constexpr (ROWPAR) g = rowc[i];
-    const bool rvalid = g.valid > 0, inrange = g.valid >= 0;
-    T* x = tile + (size_t)(inrange ? i : 0) * V;
-    T xb = 0, xy = 0;
-    if (rvalid) {
-        xb = x[d.blank];
-        xy = x[g.y >= 0 ? g.y : 0];
-    }
-    __syncwarp();
-    Pair* x2 = reinterpret_cast<Pair*>(x);
-    if (rvalid) {
-        if ((V & 1) == 0) {   // pairs: one shared-memory load and one store per two elements
-#pragma unroll 4
-            for (int p = h; p < (V >> 1); p += TPR) {
-                Pair v = x2[p];
-                v.x = R::exp2(fma(v.x - g.m, (T)R::kLog2e, g.cA));
-                v.y = R::exp2(fma(v.y - g.m, (T)R::kLog2e, g.cA));
-                if (REG) v.x = clip_grad(v.x, reg.clamp), v.y = clip_grad(v.y, reg.clamp);
-                if (SCALED) v.x *= g.scale, v.y *= g.scale;
-                x2[p] = v;
-            }
-        } else {
-#pragma unroll 4
-            for (int k = h; k < V; k += TPR) {
-                T e = R::exp2(fma(x[k] - g.m, (T)R::kLog2e, g.cA));
-                if (REG) e = clip_grad(e, reg.clamp);
-                if (SCALED) e *= g.scale;
-                x[k] = e;
-            }
-        }
-    } else if (inrange) {
-        for (int k = h; k < V; k += TPR) x[k] = T(0);
-    }
-    __syncwarp();
-    if (rvalid && h == 0) {
-        if constexpr (REG) {
-            // the sweep stored clip(dense) at the blank and label words; the clip belongs to the corrected
-            // value, so both words are rewritten from the dense term minus their corrections
-            T gb = R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cA)) - R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cB));
-            if (g.y == d.blank) gb -= R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
-            gb = clip_grad(gb, reg.clamp);
-            if (SCALED) gb *= g.scale;
-            x[d.blank] = gb;
-            if (g.y >= 0 && g.y != d.blank) {
-                T gl = R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cA)) - R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
-                gl = clip_grad(gl, reg.clamp);
-                if (SCALED) gl *= g.scale;
-                x[g.y] = gl;
-            }
-        } else {
-            T gb = R::exp2(fma(xb - g.m, (T)R::kLog2e, g.cB));
-            if (SCALED) gb *= g.scale;
-            x[d.blank] -= gb;
-            if (g.y >= 0) {
-                T gl = R::exp2(fma(xy - g.m, (T)R::kLog2e, g.cL));
-                if (SCALED) gl *= g.scale;
-                x[g.y] -= gl;
-            }
-        }
-    }
-    if (bulk) {
-        fence_async_smem();   // generic-proxy writes -> visible to the bulk copy engine
-        __syncthreads();
-        if (threadIdx.x == 0) bulk_s2g_and_wait(gout, smem_u32(tile), nelem * (uint32_t)sizeof(T));
-    } else {
-        __syncthreads();
-        for (uint32_t k = threadIdx.x; k < nelem; k += NT) gout[k] = tile[k];
-    }
-}
-template <typename T, int TPR, int NT, bool SCALED, bool REG>
-__global__ void __launch_bounds__(NT)
-grad_chunk_pruned_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
-                         const int* __restrict__ xlen, const int* __restrict__ ylen,
-                         const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                         const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
-                         const T scale_in, const T* __restrict__ scale_vec, const Dims d, const int hmajor,
-                         const uint32_t wait_ns, const GradReg<T> reg, const Prune p) {
-    grad_chunk<T, TPR, NT, SCALED, REG, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf, scale_in,
-                                              scale_vec, d, hmajor, wait_ns, reg, &p);
 }
 
 }  // namespace b200rnnt

@@ -382,10 +382,18 @@ struct Group {
     GradReg<T> gr;
     cudaStream_t s;      // the call's stream (the grouped schedule runs each lattice on a side stream)
     bool pdl;            // launch the dependent kernels with programmatic stream serialization
-    bool pruned;         // the *_pruned_kernel instantiations, given `pr`
+    bool pruned;         // the PRUNED streaming kernels, given `pr` (the dense ones get ranges == NULL)
     Prune pr;
     bool scaled() const { return scale != T(1) || scale_vec; }
 };
+
+// Calls f with one std::integral_constant<bool, ...> per flag, in order: each kernel choice becomes a template
+// argument in one place, and the launch sites below name every streaming kernel once.
+template <typename F> void with_flags(F&& f) { f(); }
+template <typename F, typename... Flags> void with_flags(F&& f, bool first, Flags... rest) {
+    if (first) with_flags([&](auto... c) { f(std::true_type{}, c...); }, rest...);
+    else with_flags([&](auto... c) { f(std::false_type{}, c...); }, rest...);
+}
 
 // ---- streaming-kernel dispatch on (vector width, row length) -------------------------------------
 // Long rows: one CTA per row (grid = rows).  Short rows: register tiles, 32/LPR rows per warp.
@@ -394,33 +402,18 @@ struct Group {
 template <typename T, int VEC, int NV, typename IO>
 void launch_row(const Group<T, IO>& g, int pass) {
     using Val = const typename Lat<T>::val*;
-    if (g.pruned) {
-        if (pass == 1) {
-            rowstats_row_pruned_kernel<T, VEC, NV, IO><<<g.d.rows, RowThreads<IO>::value, 0, g.s>>>(
+    with_flags([&](auto scaled, auto reg, auto pruned) {
+        constexpr bool SCALED = decltype(scaled)::value, REG = decltype(reg)::value, PRUNED = decltype(pruned)::value;
+        if (pass == 1)
+            rowstats_row_kernel<T, VEC, NV, IO, PRUNED><<<g.d.rows, RowThreads<IO>::value, 0, g.s>>>(
                 g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
                 static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d, g.pr);
-        } else {
-            auto k = g.reg ? (g.scaled() ? grad_row_pruned_kernel<T, VEC, NV, true, IO, true>
-                                         : grad_row_pruned_kernel<T, VEC, NV, false, IO, true>)
-                           : (g.scaled() ? grad_row_pruned_kernel<T, VEC, NV, true, IO, false>
-                                         : grad_row_pruned_kernel<T, VEC, NV, false, IO, false>);
-            launch_k(k, dim3(g.d.rows), dim3(RowThreads<IO>::value), 0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen,
-                     g.ylen, static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
+        else
+            launch_k(grad_row_kernel<T, VEC, NV, SCALED, IO, REG, PRUNED>, dim3(g.d.rows), dim3(RowThreads<IO>::value),
+                     0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen,
+                     static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
                      static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
-        }
-    } else if (pass == 1) {
-        rowstats_row_kernel<T, VEC, NV, IO><<<g.d.rows, RowThreads<IO>::value, 0, g.s>>>(
-            g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
-            static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d);
-    } else {
-        auto k = g.reg ? (g.scaled() ? grad_row_kernel<T, VEC, NV, true, IO, true>
-                                     : grad_row_kernel<T, VEC, NV, false, IO, true>)
-                       : (g.scaled() ? grad_row_kernel<T, VEC, NV, true, IO>
-                                     : grad_row_kernel<T, VEC, NV, false, IO>);
-        launch_k(k, dim3(g.d.rows), dim3(RowThreads<IO>::value), 0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen,
-                 g.ylen, static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
-                 static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr);
-    }
+    }, g.scaled(), g.reg, g.pruned);
     ++g_last_launches;
 }
 
@@ -429,33 +422,18 @@ void launch_tile(const Group<T, IO>& g, int pass) {
     using Val = const typename Lat<T>::val*;
     const uint64_t warps = ((uint64_t)g.d.rows * LPR + 31) / 32;
     const unsigned grid = (unsigned)((warps + 7) / 8);
-    if (g.pruned) {
-        if (pass == 1) {
-            rowstats_tile_pruned_kernel<T, VEC, LPR, IO><<<grid, 256, 0, g.s>>>(
+    with_flags([&](auto scaled, auto reg, auto pruned) {
+        constexpr bool SCALED = decltype(scaled)::value, REG = decltype(reg)::value, PRUNED = decltype(pruned)::value;
+        if (pass == 1)
+            rowstats_tile_kernel<T, VEC, LPR, IO, PRUNED><<<grid, 256, 0, g.s>>>(
                 g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
                 static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d, g.pr);
-        } else {
-            auto k = g.reg ? (g.scaled() ? grad_tile_pruned_kernel<T, VEC, LPR, true, IO, true>
-                                         : grad_tile_pruned_kernel<T, VEC, LPR, false, IO, true>)
-                           : (g.scaled() ? grad_tile_pruned_kernel<T, VEC, LPR, true, IO, false>
-                                         : grad_tile_pruned_kernel<T, VEC, LPR, false, IO, false>);
-            launch_k(k, dim3(grid), dim3(256), 0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen,
-                     static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
-                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
-        }
-    } else if (pass == 1) {
-        rowstats_tile_kernel<T, VEC, LPR, IO><<<grid, 256, 0, g.s>>>(
-            g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
-            static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d);
-    } else {
-        auto k = g.reg ? (g.scaled() ? grad_tile_kernel<T, VEC, LPR, true, IO, true>
-                                     : grad_tile_kernel<T, VEC, LPR, false, IO, true>)
-                       : (g.scaled() ? grad_tile_kernel<T, VEC, LPR, true, IO>
-                                     : grad_tile_kernel<T, VEC, LPR, false, IO>);
-        launch_k(k, dim3(grid), dim3(256), 0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen,
-                 static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
-                 static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr);
-    }
+        else
+            launch_k(grad_tile_kernel<T, VEC, LPR, SCALED, IO, REG, PRUNED>, dim3(grid), dim3(256), 0, g.s, g.pdl,
+                     g.acts, g.grads, g.labels, g.xlen, g.ylen, static_cast<const typename Real<T>::pair*>(g.w.stat),
+                     static_cast<Val>(g.w.alphas), static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale,
+                     g.scale_vec, g.d, g.gr, g.pr);
+    }, g.scaled(), g.reg, g.pruned);
     ++g_last_launches;
 }
 
@@ -568,35 +546,19 @@ bool chunk_pass(const Group<T, T>& g, int pass) {
     auto go = [&](auto tpr_c, auto nt_c) {
         constexpr int TPR = decltype(tpr_c)::value, NT = decltype(nt_c)::value;
         if constexpr (NT / TPR >= 4) {
-            if (g.pruned) {
-                if (pass == 1) {
-                    prefer_smem(rowstats_chunk_pruned_kernel<T, TPR, NT>)<<<grid, NT, smem, g.s>>>(
+            with_flags([&](auto scaled, auto reg, auto pruned) {
+                constexpr bool SCALED = decltype(scaled)::value, REG = decltype(reg)::value;
+                constexpr bool PRUNED = decltype(pruned)::value;
+                if (pass == 1)
+                    prefer_smem(rowstats_chunk_kernel<T, TPR, NT, PRUNED>)<<<grid, NT, smem, g.s>>>(
                         g.acts, g.labels, g.xlen, g.ylen, static_cast<Pair*>(g.w.stat), static_cast<Fac*>(g.w.lp2), g.d,
                         hmajor, wait_ns, g.pr);
-                } else {
-                    auto k = g.reg ? (g.scaled() ? grad_chunk_pruned_kernel<T, TPR, NT, true, true>
-                                                 : grad_chunk_pruned_kernel<T, TPR, NT, false, true>)
-                                   : (g.scaled() ? grad_chunk_pruned_kernel<T, TPR, NT, true, false>
-                                                 : grad_chunk_pruned_kernel<T, TPR, NT, false, false>);
-                    launch_k(prefer_smem(k), dim3(grid), dim3(NT), smem, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen,
-                             g.ylen, static_cast<const Pair*>(g.w.stat), static_cast<const Val*>(g.w.alphas),
-                             static_cast<const Val*>(g.w.betas), static_cast<const Val*>(g.w.llf), g.scale,
-                             g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr);
-                }
-            } else if (pass == 1)
-                prefer_smem(rowstats_chunk_kernel<T, TPR, NT>)<<<grid, NT, smem, g.s>>>(
-                    g.acts, g.labels, g.xlen, g.ylen, static_cast<Pair*>(g.w.stat), static_cast<Fac*>(g.w.lp2), g.d,
-                    hmajor, wait_ns);
-            else {
-                auto k = g.reg ? (g.scaled() ? grad_chunk_kernel<T, TPR, NT, true, true>
-                                             : grad_chunk_kernel<T, TPR, NT, false, true>)
-                               : (g.scaled() ? grad_chunk_kernel<T, TPR, NT, true>
-                                             : grad_chunk_kernel<T, TPR, NT, false>);
-                launch_k(prefer_smem(k), dim3(grid), dim3(NT), smem, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen,
-                         g.ylen, static_cast<const Pair*>(g.w.stat), static_cast<const Val*>(g.w.alphas),
-                         static_cast<const Val*>(g.w.betas), static_cast<const Val*>(g.w.llf), g.scale, g.scale_vec, g.d,
-                         hmajor, wait_ns, g.gr);
-            }
+                else
+                    launch_k(prefer_smem(grad_chunk_kernel<T, TPR, NT, SCALED, REG, PRUNED>), dim3(grid), dim3(NT), smem,
+                             g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, static_cast<const Pair*>(g.w.stat),
+                             static_cast<const Val*>(g.w.alphas), static_cast<const Val*>(g.w.betas),
+                             static_cast<const Val*>(g.w.llf), g.scale, g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr);
+            }, g.scaled(), g.reg, g.pruned);
         }
     };
     auto with_rpt = [&](auto tpr_c) {

@@ -67,25 +67,23 @@ __device__ __forceinline__ void utt_extent(const Dims& d, const int* __restrict_
 }
 
 // ---- pruned logits (DESIGN.md §8) -----------------------------------------------------------------------
-// The streaming kernels come in a dense and a PRUNED instantiation.  Pruned logits are [N, maxT, R, V]: row
-// (b, t, s) holds lattice cell (t, u = ranges[b*maxT + t] + s), and Dims.rows counts those rows.  The window
-// starts and R travel beside Dims, not in it, so the dense instantiations do not change.
+// Each streaming kernel takes `bool PRUNED` as its last template parameter and a Prune by value as its last
+// argument.  Pruned logits are [N, maxT, R, V]: row (b, t, s) holds lattice cell (t, u = ranges[b*maxT + t] + s),
+// and Dims.rows counts those rows.  The dense instantiations get ranges == NULL and never read the Prune.
 struct Prune {
     const int* ranges;   // [N, maxT] window start per frame (any int32)
     FastDiv divR;        // R = rows per frame
 };
-// row -> (b, t, u); p is NULL in the dense instantiations (the kernels' bodies take Dims by value and the
-// windows by pointer: that keeps the dense instantiations' SASS exactly what it was before the bodies were
-// shared).  Pruned: u is ranges + s in 32-bit two's complement; a negative or too large u lands at or
+// row -> (b, t, u).  Pruned: u is ranges + s in 32-bit two's complement; a negative or too large u lands at or
 // above 2^31 as unsigned, where row_padding() catches it together with u >= U_b
 template <bool PRUNED>
-__device__ __forceinline__ void row_decode(const Dims& d, const Prune* p, uint32_t r, uint32_t& b, uint32_t& t,
+__device__ __forceinline__ void row_decode(const Dims& d, const Prune& p, uint32_t r, uint32_t& b, uint32_t& t,
                                            uint32_t& u) {
     if constexpr (PRUNED) {
         uint32_t bt, s;
-        p->divR.divmod(r, bt, s);
+        p.divR.divmod(r, bt, s);
         d.divT.divmod(bt, b, t);
-        u = (uint32_t)__ldg(p->ranges + bt) + s;
+        u = (uint32_t)__ldg(p.ranges + bt) + s;
     } else {
         d.decode(r, b, t, u);
     }
@@ -98,11 +96,13 @@ template <bool PRUNED> __device__ __forceinline__ bool row_padding(uint32_t t, u
 // pruned instantiations ask: a dense lattice always has a path.
 __device__ __forceinline__ bool ll_dead(const LogVal* llf, uint32_t b) { return llf[b].e < kEDead; }
 __device__ __forceinline__ bool ll_dead(const double* llf, uint32_t b) { return llf[b] == -(double)INFINITY; }
-// padding of pass 2: row_padding, and in the pruned instantiations also every row of an utterance without a path
-template <bool PRUNED, typename Val>
-__device__ __forceinline__ bool grad_padding(uint32_t t, uint32_t u, int Tb, int Ub, const Val* llf, uint32_t b) {
-    if constexpr (PRUNED) return row_padding<true>(t, u, Tb, Ub) || ll_dead(llf, b);
-    else return row_padding<false>(t, u, Tb, Ub);
+// padding of pass 2 in the pruned instantiations: row_padding, and every row of an utterance without a path.  The
+// dense instantiations spell out their test, t >= T_b or u >= U_b, where they use it: returned from a helper, it
+// compiled to other index code in every dense gradient kernel, and grad_row_kernel<float, 4, 5> (C3) ran 0.9 %
+// slower (H100 80GB HBM3, 400 W).
+template <typename Val>
+__device__ __forceinline__ bool pruned_grad_padding(uint32_t t, uint32_t u, int Tb, int Ub, const Val* llf, uint32_t b) {
+    return row_padding<true>(t, u, Tb, Ub) || ll_dead(llf, b);
 }
 
 // Pruned calls start from log-zero factors everywhere, so that a cell no row covers has neither transition; pass 1
@@ -131,10 +131,11 @@ template <typename IO> struct RowThreads { static constexpr int value = sizeof(I
 #define RNNT_ROWSTATS_MINB 7
 #endif
 template <typename T, int VEC, int NV, typename IO, bool PRUNED>
-__device__ __forceinline__ void rowstats_row(const IO* __restrict__ acts, const int* __restrict__ labels,
-                                             const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                             typename Real<T>::pair* __restrict__ stat,
-                                             typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune* p) {
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_ROWSTATS_MINB : 8))
+rowstats_row_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
+                    const int* __restrict__ xlen, const int* __restrict__ ylen,
+                    typename Real<T>::pair* __restrict__ stat, typename Lat<T>::fac* __restrict__ lp2,
+                    const Dims d, const Prune p) {
     using R = Real<T>;
     constexpr int kRowThreads = RowThreads<IO>::value;
     __shared__ T sh_m[kRowThreads / 32], sh_s[kRowThreads / 32];
@@ -252,22 +253,6 @@ __device__ __forceinline__ void rowstats_row(const IO* __restrict__ acts, const 
         }
     }
 }
-template <typename T, int VEC, int NV, typename IO = T>
-__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_ROWSTATS_MINB : 8))
-rowstats_row_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
-                    const int* __restrict__ xlen, const int* __restrict__ ylen,
-                    typename Real<T>::pair* __restrict__ stat, typename Lat<T>::fac* __restrict__ lp2,
-                    const Dims d) {
-    rowstats_row<T, VEC, NV, IO, false>(acts, labels, xlen, ylen, stat, lp2, d, nullptr);
-}
-template <typename T, int VEC, int NV, typename IO>
-__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_ROWSTATS_MINB : 8))
-rowstats_row_pruned_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
-                           const int* __restrict__ xlen, const int* __restrict__ ylen,
-                           typename Real<T>::pair* __restrict__ stat, typename Lat<T>::fac* __restrict__ lp2,
-                           const Dims d, const Prune p) {
-    rowstats_row<T, VEC, NV, IO, true>(acts, labels, xlen, ylen, stat, lp2, d, &p);
-}
 
 // =================================================================================================
 // Pass 1, short rows (V/VEC <= 8*LPR): the whole row lives in registers — each of the LPR lanes
@@ -282,10 +267,11 @@ rowstats_row_pruned_kernel(const IO* __restrict__ acts, const int* __restrict__ 
 constexpr int kVPL = RNNT_VPL;
 
 template <typename T, int VEC, int LPR, typename IO, bool PRUNED>
-__device__ __forceinline__ void rowstats_tile(const IO* __restrict__ acts, const int* __restrict__ labels,
-                                              const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                              typename Real<T>::pair* __restrict__ stat,
-                                              typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune* p) {
+__global__ void __launch_bounds__(256)
+rowstats_tile_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
+                     const int* __restrict__ xlen, const int* __restrict__ ylen,
+                     typename Real<T>::pair* __restrict__ stat,
+                     typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p) {
     using R = Real<T>;
     constexpr int RPW = kWarp / LPR;
     const int lane = threadIdx.x & 31;
@@ -346,22 +332,6 @@ __device__ __forceinline__ void rowstats_tile(const IO* __restrict__ acts, const
             lp2[skew(d, b, t, u)] = Lat<T>::make(lpb, lpl, has_label);
         }
     }
-}
-template <typename T, int VEC, int LPR, typename IO = T>
-__global__ void __launch_bounds__(256)
-rowstats_tile_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
-                     const int* __restrict__ xlen, const int* __restrict__ ylen,
-                     typename Real<T>::pair* __restrict__ stat,
-                     typename Lat<T>::fac* __restrict__ lp2, const Dims d) {
-    rowstats_tile<T, VEC, LPR, IO, false>(acts, labels, xlen, ylen, stat, lp2, d, nullptr);
-}
-template <typename T, int VEC, int LPR, typename IO>
-__global__ void __launch_bounds__(256)
-rowstats_tile_pruned_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
-                            const int* __restrict__ xlen, const int* __restrict__ ylen,
-                            typename Real<T>::pair* __restrict__ stat,
-                            typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p) {
-    rowstats_tile<T, VEC, LPR, IO, true>(acts, labels, xlen, ylen, stat, lp2, d, &p);
 }
 
 // =================================================================================================
@@ -740,18 +710,14 @@ __device__ __forceinline__ RowGrad<float> row_grad_setup_spec(const Dims& d, uin
 #ifndef RNNT_GRAD_MINB16
 #define RNNT_GRAD_MINB16 8   // 16-bit rows are one trip of 128 threads: residency (bytes in flight) is what pays
 #endif
-// The pass-2 bodies are instantiated for the pruned kernels only: the dense gradient kernels below keep their own
-// text, because compiled through a shared body their SASS changed (same instructions, another register
-// allocation and order).  PRUNED = false here is the dense kernel's code, line for line.
 template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED>
-__device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                                         const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                         const typename Real<T>::pair* __restrict__ stat,
-                                         const typename Lat<T>::val* __restrict__ alphas,
-                                         const typename Lat<T>::val* __restrict__ betas,
-                                         const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                                         const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
-                                         const Prune* p) {
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
+grad_row_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                const int* __restrict__ xlen, const int* __restrict__ ylen,
+                const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                const Prune p) {
     constexpr int kRowThreads = RowThreads<IO>::value;
     const uint32_t r = d.rows - 1 - blockIdx.x;
     uint32_t u, b, t;
@@ -764,7 +730,7 @@ __device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __rest
     IO* grow = grads + (uint64_t)r * d.V;
     // per-utterance upstream gradient (autograd's grad_output) times the scalar factor
     const T scale = (SCALED && scale_vec) ? __ldg(scale_vec + b) * scale_in : scale_in;
-    if (grad_padding<PRUNED>(t, u, Tb, Ub, llf, b)) {
+    if (PRUNED ? pruned_grad_padding(t, u, Tb, Ub, llf, b) : (int)t >= Tb || (int)u >= Ub) {
         VecT<T, VEC> z;
 #pragma unroll
         for (int c = 0; c < VEC; ++c) z.v[c] = 0;
@@ -807,93 +773,17 @@ __device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __rest
         load(base);
         emit(base);
     }
-}
-template <typename T, int VEC, int NV, bool SCALED, typename IO = T, bool REG = false>
-__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
-grad_row_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                const int* __restrict__ xlen, const int* __restrict__ ylen,
-                const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                const T* __restrict__ scale_vec,
-                const Dims d, const GradReg<T> reg) {
-    constexpr int kRowThreads = RowThreads<IO>::value;
-    const uint32_t r = d.rows - 1 - blockIdx.x;
-    uint32_t u, b, t;
-    d.decode(r, b, t, u);
-    int Tb, Ub;
-    utt_extent(d, xlen, ylen, b, Tb, Ub);
-    const int nv = d.V / VEC;
-    const int kb = d.blank;
-    const IO* row = acts + (uint64_t)r * d.V;
-    IO* grow = grads + (uint64_t)r * d.V;
-    // per-utterance upstream gradient (autograd's grad_output) times the scalar factor
-    const T scale = (SCALED && scale_vec) ? __ldg(scale_vec + b) * scale_in : scale_in;
-    if ((int)t >= Tb || (int)u >= Ub) {
-        VecT<T, VEC> z;
-#pragma unroll
-        for (int c = 0; c < VEC; ++c) z.v[c] = 0;
-        for (int i = threadIdx.x; i < nv; i += kRowThreads) st_stream<T, VEC>(grow + (size_t)i * VEC, z);
-        return;
-    }
-    // the logits stay PACKED in registers until they are used (16-bit storage: 20 registers instead of 40)
-    using P = typename Pack<sizeof(IO) * VEC>::type;
-    P x[NV];
-    auto load = [&](int base) {
-#pragma unroll
-        for (int j = 0; j < NV; ++j) {
-            const int i = base + j * kRowThreads;
-            if (i < nv) x[j] = __ldcs(reinterpret_cast<const P*>(row + (size_t)i * VEC));
-        }
-    };
-    load(threadIdx.x);  // in flight before the lattice constants are fetched
-    pdl_wait();         // (PDL) the logits were read ahead of the lattice kernel's completion; its output is not
-    RowGrad<T> rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
-    if constexpr (REG) fastemit_fold(rg, reg, b, t, u, d);
-    // 16-bit storage: fold the row maximum into the three offsets, one FFMA per element instead of FADD + FFMA
-    // (its rounding, |m| * 6e-8 in the exponent, is far below the 16-bit quantisation of input and output)
-    constexpr bool ZEROM = sizeof(IO) == 2;
-    if (ZEROM) {
-        const T shift = -rg.m * (T)Real<T>::kLog2e;
-        rg.cA += shift, rg.cB += shift, rg.cL += shift;
-    }
-    auto emit = [&](int base) {
-#pragma unroll
-        for (int j = 0; j < NV; ++j) {
-            const int i = base + j * kRowThreads;
-            if (i < nv)
-                st_stream<T, VEC>(grow + (size_t)i * VEC,
-                                  grad_vec<T, VEC, SCALED, ZEROM, REG>(unpack<T, VEC, IO, P>(x[j]), rg, i * VEC, kb,
-                                                                       scale, reg.clamp));
-        }
-    };
-    emit(threadIdx.x);
-    for (int base = threadIdx.x + kRowThreads * NV; base < nv; base += kRowThreads * NV) {  // V > 256*NV*VEC only
-        load(base);
-        emit(base);
-    }
-}
-template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG>
-__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
-grad_row_pruned_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                       const int* __restrict__ xlen, const int* __restrict__ ylen,
-                       const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                       const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
-                       const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
-                       const Prune p) {
-    grad_row<T, VEC, NV, SCALED, IO, REG, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf, scale_in,
-                                                scale_vec, d, reg, &p);
 }
 
 // Pass 2, short rows: same register tile as rowstats_tile_kernel.
 template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED>
-__device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                                          const int* __restrict__ xlen, const int* __restrict__ ylen,
-                                          const typename Real<T>::pair* __restrict__ stat,
-                                          const typename Lat<T>::val* __restrict__ alphas,
-                                          const typename Lat<T>::val* __restrict__ betas,
-                                          const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                                          const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
-                                          const Prune* p) {
+__global__ void __launch_bounds__(256)
+grad_tile_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                 const int* __restrict__ xlen, const int* __restrict__ ylen,
+                 const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                 const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                 const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                 const Prune p) {
     constexpr int RPW = kWarp / LPR;
     const int lane = threadIdx.x & 31;
     const int sub = lane / LPR, sl = lane % LPR;
@@ -912,7 +802,7 @@ __device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __res
         const IO* row = acts + (uint64_t)r * d.V;
         IO* grow = grads + (uint64_t)r * d.V;
         const T scale = (SCALED && scale_vec) ? __ldg(scale_vec + b) * scale_in : scale_in;
-        if (grad_padding<PRUNED>(t, u, Tb, Ub, llf, b)) {
+        if (PRUNED ? pruned_grad_padding(t, u, Tb, Ub, llf, b) : (int)t >= Tb || (int)u >= Ub) {
             VecT<T, VEC> z;
 #pragma unroll
             for (int c = 0; c < VEC; ++c) z.v[c] = 0;
@@ -940,72 +830,6 @@ __device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __res
                                   grad_vec<T, VEC, SCALED, false, REG>(x[j], rg, i * VEC, kb, scale, reg.clamp));
         }
     } while (false);
-}
-template <typename T, int VEC, int LPR, bool SCALED, typename IO = T, bool REG = false>
-__global__ void __launch_bounds__(256)
-grad_tile_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                 const int* __restrict__ xlen, const int* __restrict__ ylen,
-                 const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                 const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf, const T scale_in,
-                const T* __restrict__ scale_vec,
-                 const Dims d, const GradReg<T> reg) {
-    constexpr int RPW = kWarp / LPR;
-    const int lane = threadIdx.x & 31;
-    const int sub = lane / LPR, sl = lane % LPR;
-    const uint64_t gw = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int nv = d.V / VEC;
-    const int kb = d.blank;
-
-    do {   // non-persistent: one tile of RPW rows per warp
-        const uint64_t rr = gw * RPW + sub;
-        if (rr >= d.rows) continue;
-        const uint32_t r = d.rows - 1 - (uint32_t)rr;
-        uint32_t u, b, t;
-        d.decode(r, b, t, u);
-        int Tb, Ub;
-        utt_extent(d, xlen, ylen, b, Tb, Ub);
-        const IO* row = acts + (uint64_t)r * d.V;
-        IO* grow = grads + (uint64_t)r * d.V;
-        const T scale = (SCALED && scale_vec) ? __ldg(scale_vec + b) * scale_in : scale_in;
-        if ((int)t >= Tb || (int)u >= Ub) {
-            VecT<T, VEC> z;
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) z.v[c] = 0;
-#pragma unroll
-            for (int j = 0; j < kVPL; ++j) {
-                const int i = sl + j * LPR;
-                if (i < nv) st_stream<T, VEC>(grow + (size_t)i * VEC, z);
-            }
-            continue;
-        }
-        VecT<T, VEC> x[kVPL];
-#pragma unroll
-        for (int j = 0; j < kVPL; ++j) {
-            const int i = sl + j * LPR;
-            if (i < nv) x[j] = ld_stream<T, VEC>(row + (size_t)i * VEC);
-        }
-        pdl_wait();
-        RowGrad<T> rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
-        if constexpr (REG) fastemit_fold(rg, reg, b, t, u, d);
-#pragma unroll
-        for (int j = 0; j < kVPL; ++j) {
-            const int i = sl + j * LPR;
-            if (i < nv)
-                st_stream<T, VEC>(grow + (size_t)i * VEC,
-                                  grad_vec<T, VEC, SCALED, false, REG>(x[j], rg, i * VEC, kb, scale, reg.clamp));
-        }
-    } while (false);
-}
-template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG>
-__global__ void __launch_bounds__(256)
-grad_tile_pruned_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                        const int* __restrict__ xlen, const int* __restrict__ ylen,
-                        const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                        const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
-                        const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
-                        const Prune p) {
-    grad_tile<T, VEC, LPR, SCALED, IO, REG, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf, scale_in,
-                                                  scale_vec, d, reg, &p);
 }
 
 }  // namespace b200rnnt
