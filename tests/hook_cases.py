@@ -1,10 +1,12 @@
 """Child process of test_gpu_tuning_hooks.py: runs one suite of shapes through the library with the tuning hooks
 (RNNT_B200_* environment variables, README) already set in its environment, and checks each against the fp64 oracle.
 
-    python tests/hook_cases.py {dense|joint|smoothed} OUT_DIR
+    python tests/hook_cases.py {dense|joint|smoothed|pruned} OUT_DIR
 
 "smoothed" runs the JOINT shapes with lm_only_scale 0.25 and am_only_scale 0.1 (DESIGN.md §9) and checks them
-against the closed-form fp64 reference (tests/smoothed_reference.py).
+against the closed-form fp64 reference (tests/smoothed_reference.py).  "pruned" runs the DENSE shapes as pruned
+calls (DESIGN.md §8) with R = 3 rows per frame over windows from random_monotone_ranges, and checks them against
+the fp64 reference (tests/pruned_reference.py).
 
 A hook is read once per process into a static, so every hook setting needs a process of its own.  Saves each
 shape's costs and gradients to OUT_DIR/<shape>.npz and prints one JSON line:
@@ -27,6 +29,7 @@ for p in (ROOT, os.path.join(ROOT, "warp-transducer_b200"), os.path.dirname(os.p
 import torch  # noqa: E402
 from torch.profiler import ProfilerActivity, profile  # noqa: E402
 
+import pruned_reference  # noqa: E402
 import smoothed_reference  # noqa: E402
 from joint_reference import grad_mismatch, reference as joint_reference  # noqa: E402
 from oracle import pyoracle  # noqa: E402
@@ -53,9 +56,10 @@ SMOOTH = (0.25, 0.1)   # (lm_only_scale, am_only_scale) of the smoothed suite
 # per shape where a hook needs more.  U8_V5121: RNNT_B200_JOINT_SLICES=1 sums all 5121 columns of S in one
 # tensor-core accumulation instead of 16 slabs; measured 1.79e-7 on an H100 80GB HBM3 at 700 W.
 SMOOTH_FLOOR_DENSE = {"U8_V5121": 3e-7}
+PRUNED_R = 3   # rows per frame of the pruned suite
 
 
-def inputs(name, shape, joint):
+def inputs(name, shape, joint, pruned=False):
     seed = sum(map(ord, name))
     rng = np.random.default_rng(seed)
     N, T, U, V = shape
@@ -65,6 +69,12 @@ def inputs(name, shape, joint):
     tl[0], ul[0] = T, U - 1
     if joint:
         x = ((rng.standard_normal((N, T, V)) * 2).astype(np.float32), (rng.standard_normal((N, U, V)) * 2).astype(np.float32))
+    elif pruned:
+        # utterance 0 keeps U_b = U, without a path where R - 1 labels per frame cannot reach it (U301: dead chains
+        # across every warp of the wavefront); the others are cut to what their windows can reach
+        ul[1:] = np.minimum(ul[1:], (tl[1:] - 1) * (PRUNED_R - 1))
+        ranges = pruned_reference.random_monotone_ranges(rng, tl, ul, T, PRUNED_R)
+        x = ((rng.standard_normal((N, T, PRUNED_R, V)) * 2).astype(np.float32), ranges)
     else:
         x = (rng.standard_normal((N, T, U, V)) * 2).astype(np.float32)
     return x, labels, tl, ul
@@ -81,6 +91,42 @@ def run_dense(wr, acts, labels, tl, ul):
     torch.cuda.synchronize()
     del ws
     return costs.cpu().numpy(), grads.cpu().numpy(), launches
+
+
+def run_pruned(wr, logits, ranges, labels, tl, ul, U):
+    """The full pruned call (rnnt_b200_pruned_loss_async_ex) over the whole lattice width U."""
+    from warprnnt_pytorch.pruned import pruned_workspace_size
+    N, T, R, V = logits.shape
+    x = torch.tensor(logits, device="cuda")
+    rg, lab, tld, uld = (torch.as_tensor(a).cuda() for a in (ranges, labels, tl, ul))
+    costs = torch.empty(N, device="cuda")
+    grads = torch.full_like(x, float("nan"))
+    ws = torch.empty(pruned_workspace_size(T, U, R, N, 4), dtype=torch.uint8, device="cuda")
+    opt = wr.rnntOptions(loc=1, num_threads=0, stream=torch.cuda.current_stream().cuda_stream, blank_label=0,
+                         maxT=T, maxU=U, batch_first=True)
+    st = wr.lib().rnnt_b200_pruned_loss_async_ex(0, 0, x.data_ptr(), grads.data_ptr(), rg.data_ptr(), R,
+                                                 lab.data_ptr(), uld.data_ptr(), tld.data_ptr(), V, N,
+                                                 costs.data_ptr(), 1.0, wr.rnntGradOptions(0.0, 0.0), ws.data_ptr(),
+                                                 opt)
+    assert st == 0, wr.status_string(st)
+    launches = wr.last_launch_count()
+    torch.cuda.synchronize()
+    del ws
+    return costs.cpu().numpy(), grads.cpu().numpy(), launches
+
+
+def check_pruned(out, x, labels, tl, ul):
+    costs, grads = out
+    c_ref, g_ref = pruned_reference.pruned_loss(x[0].astype(np.float64), labels, tl, ul, x[1], 0)
+    problems = []
+    fin = np.isfinite(c_ref)
+    if not (np.array_equal(np.isfinite(costs), fin) and np.allclose(costs[fin], c_ref[fin], rtol=1e-5, atol=1e-5)):
+        problems.append("costs: %s against %s" % (costs.tolist(), c_ref.tolist()))
+    if np.isnan(grads).any() or not np.allclose(grads, g_ref, rtol=1e-4, atol=1e-6):
+        problems.append("grads: max |err| %.3g" % np.nanmax(np.abs(grads - g_ref)))
+    if grads[~fin].any():
+        problems.append("an utterance without a path has a gradient")
+    return problems
 
 
 def run_joint(wr, trans, pred, labels, tl, ul):
@@ -152,16 +198,24 @@ def main():
     lib.rnnt_b200_debug_policy.restype = C.c_int
     lib.rnnt_b200_debug_policy.argtypes = [C.c_int, C.c_int, C.c_int]
     joint = suite in ("joint", "smoothed")
+    pruned = suite == "pruned"
+    if pruned:
+        import warprnnt_pytorch.pruned  # noqa: F401  (argtypes of the pruned entries)
     shapes = JOINT if joint else DENSE
-    run = {"dense": run_dense, "joint": run_joint, "smoothed": run_smoothed}[suite]
+    run = {"dense": run_dense, "joint": run_joint, "smoothed": run_smoothed, "pruned": run_pruned}[suite]
     results, kernels = {}, set()
     for name, shape in shapes.items():
-        x, labels, tl, ul = inputs(name, shape, joint)
+        x, labels, tl, ul = inputs(name, shape, joint, pruned)
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            *out, launches = run(wr, *(x if joint else (x,)), labels, tl, ul)
+            if pruned:
+                *out, launches = run(wr, *x, labels, tl, ul, shape[2])
+            else:
+                *out, launches = run(wr, *(x if joint else (x,)), labels, tl, ul)
         kernels.update(e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
         if suite == "smoothed":
             problems = check_smoothed(name, out, x, labels, tl, ul)
+        elif pruned:
+            problems = check_pruned(out, x, labels, tl, ul)
         else:
             problems = (check_joint if joint else check_dense)(out, x, labels, tl, ul)
         keys = ("costs", "dF", "dG") if joint else ("costs", "grads")

@@ -81,7 +81,63 @@ CASES = {
     "GROUPS_3": ("dense", {"RNNT_B200_GROUPS": "3"}, [], [], True),
     "GROUPS_8": ("dense", {"RNNT_B200_GROUPS": "8"}, [], [], True),
     "PDL_1": ("dense", {"RNNT_B200_PDL": "1"}, [], [], True),
+    # pruned loss (DESIGN.md §8): each hook must run the PRUNED instantiation (last template argument true) it selects
+    "PRUNED_CHUNK_0": ("pruned", {"RNNT_B200_CHUNK": "0"},
+                       [r"rowstats_tile_kernel<float, 4, 2, float, true>",
+                        r"grad_tile_kernel<float, 4, 2, false, float, false, true>",
+                        r"grad_tile_kernel<float, 2, 4, false, float, false, true>",
+                        r"grad_tile_kernel<float, 4, 4, false, float, false, true>"],
+                       [r"grad_chunk_kernel", r"rowstats_chunk_kernel"], False),
+    "PRUNED_CHUNK_NT_64": ("pruned", {"RNNT_B200_CHUNK_NT": "64"},
+                           [r"rowstats_chunk_kernel<float, 2, 64, true>",
+                            r"grad_chunk_kernel<float, 2, 64, false, false, true>"],
+                           [r"grad_chunk_kernel<float, 2, 256,"], True),
+    "PRUNED_CHUNK_NT_128": ("pruned", {"RNNT_B200_CHUNK_NT": "128"},
+                            [r"rowstats_chunk_kernel<float, 2, 128, true>",
+                             r"grad_chunk_kernel<float, 2, 128, false, false, true>"],
+                            [r"grad_chunk_kernel<float, 2, 256,"], True),
+    "PRUNED_CHUNK_TPR_1": ("pruned", {"RNNT_B200_CHUNK_TPR": "1"},
+                           [r"rowstats_chunk_kernel<float, 1, 256, true>",
+                            r"grad_chunk_kernel<float, 1, 256, false, false, true>"],
+                           [r"grad_chunk_kernel<float, 2, 256,"], False),
+    "PRUNED_CHUNK_TPR_2": ("pruned", {"RNNT_B200_CHUNK_TPR": "2"},
+                           [r"grad_chunk_kernel<float, 2, 256, false, false, true>"],
+                           [r"grad_chunk_kernel<float, 4, 256,"], False),
+    "PRUNED_CHUNK_TPR_4": ("pruned", {"RNNT_B200_CHUNK_TPR": "4"},
+                           [r"rowstats_chunk_kernel<float, 4, 256, true>",
+                            r"grad_chunk_kernel<float, 4, 256, false, false, true>"],
+                           [r"grad_chunk_kernel<float, 2, 256,"], False),
+    "PRUNED_CHUNK_TPR_8": ("pruned", {"RNNT_B200_CHUNK_TPR": "8"},
+                           [r"rowstats_chunk_kernel<float, 8, 256, true>",
+                            r"grad_chunk_kernel<float, 8, 256, false, false, true>"],
+                           [r"grad_chunk_kernel<float, 2, 256,"], False),
+    "PRUNED_CHUNK_MAP_0": ("pruned", {"RNNT_B200_CHUNK_MAP": "0"},
+                           [r"grad_chunk_kernel<float, 2, 256, false, false, true>"], [], True),
+    "PRUNED_CHUNK_MAP_1": ("pruned", {"RNNT_B200_CHUNK_MAP": "1"},
+                           [r"grad_chunk_kernel<float, 2, 256, false, false, true>"], [], True),
+    "PRUNED_LPR_32": ("pruned", {"RNNT_B200_LPR": "32"},
+                      [r"rowstats_tile_kernel<float, 4, 32, float, true>",
+                       r"grad_tile_kernel<float, 4, 32, false, float, false, true>"],
+                      [r"grad_tile_kernel<float, 4, 16,"], False),
+    "PRUNED_LAT_RING_16": ("pruned", {"RNNT_B200_LAT_RING": "16"},
+                           [r"lattice_lin_kernel<1, true, 16>",
+                            r"grad_chunk_kernel<float, 2, 256, false, false, true>"],
+                           [r"lattice_lin_kernel<1, true, 8>"], True),
+    "PRUNED_LAT_RING_32": ("pruned", {"RNNT_B200_LAT_RING": "32"},
+                           [r"lattice_lin_kernel<1, true, 32>",
+                            r"grad_chunk_kernel<float, 2, 256, false, false, true>"],
+                           [r"lattice_lin_kernel<1, true, 8>"], True),
+    "PRUNED_GROUPS_2": ("pruned", {"RNNT_B200_GROUPS": "2"},
+                        [r"grad_chunk_kernel<float, 2, 256, false, false, true>"], [], True),
+    "PRUNED_GROUPS_3": ("pruned", {"RNNT_B200_GROUPS": "3"},
+                        [r"grad_chunk_kernel<float, 2, 256, false, false, true>"], [], True),
+    "PRUNED_GROUPS_8": ("pruned", {"RNNT_B200_GROUPS": "8"},
+                        [r"grad_chunk_kernel<float, 2, 256, false, false, true>"], [], True),
+    "PRUNED_PDL_1": ("pruned", {"RNNT_B200_PDL": "1"},
+                     [r"grad_chunk_kernel<float, 2, 256, false, false, true>"], [], True),
 }
+STREAMING = ("rowstats_chunk_kernel", "rowstats_tile_kernel", "rowstats_row_kernel", "grad_chunk_kernel",
+             "grad_tile_kernel", "grad_row_kernel")
 
 
 def norm(name):
@@ -106,7 +162,7 @@ def run_child(suite, env_extra, out_dir):
 def baseline(tmp_path_factory):
     """The default dispatch, one child per suite (no hook set)."""
     out = {}
-    for suite in ("dense", "joint", "smoothed"):
+    for suite in ("dense", "joint", "smoothed", "pruned"):
         d = str(tmp_path_factory.mktemp("baseline_" + suite))
         out[suite] = (run_child(suite, {}, d), d)
     return out
@@ -121,6 +177,10 @@ def test_default_dispatch_matches_the_oracle(baseline):
     assert all(res["launches"] == 3 for res in dense["shapes"].values())
     assert any("grad_fused_kernel" in k for k in baseline["joint"][0]["kernels"])
     assert any("grad_fused_kernel<32, 32, 3, true>" in k for k in baseline["smoothed"][0]["kernels"])
+    pruned = baseline["pruned"][0]
+    assert all(res["launches"] == 4 for res in pruned["shapes"].values())   # the log-zero fill, then the three
+    streaming = [k.split("(")[0] for k in pruned["kernels"] if any(f in k for f in STREAMING)]
+    assert len(streaming) == 6 and all(k.endswith(", true>") for k in streaming), streaming
 
 
 @pytest.mark.parametrize("case", list(CASES))
@@ -146,7 +206,8 @@ def test_hook(case, baseline, tmp_path):
         assert all(pol[k] == int(value) for k in pol if k.startswith("map_V"))
         assert maps, "no shape whose default mapping differs from the forced one"
     elif key == "RNNT_B200_GROUPS":
-        assert all(res["launches"] == 3 * int(value) for res in rep["shapes"].values()), rep["shapes"]
+        fill = 1 if suite == "pruned" else 0   # a pruned call fills the whole lattice once, before every group
+        assert all(res["launches"] == fill + 3 * int(value) for res in rep["shapes"].values()), rep["shapes"]
     elif key == "RNNT_B200_PDL":
         assert pol["pdl"] == 1
     elif key == "RNNT_B200_LAT_RING":
