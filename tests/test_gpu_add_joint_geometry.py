@@ -73,7 +73,10 @@ SHAPES = {
     "T1500_fused_47_chunks_V129": (1, 1500, 24, 129, 0),
     # two-kernel gradient: dG with K = T = 1000; dF with N = T = 1000 in 16 tiles of 64, MODE 3
     "U40_T1000_long_K_dG_16_dF_tiles": (1, 1000, 40, 64, 0),
+    # S with both M and N tiled: 3 M tiles of frames (the last of 4 rows) x 2 N tiles of label positions (128 + 23)
+    "S_T260_U151_M_and_N_tiled": (1, 260, 151, 132, 0),
     # S split-K: V // 320 slabs (at most 16) of kper = ceil(V / slabs) rounded up to 32
+    "V636_one_slab_K636_MODE2": (2, 20, 6, 636, 0),          # the largest V of one slab: 20 stages, the last of 28
     "V641_MODE1_two_slabs": (2, 20, 6, 641, 0),
     "V5001_MODE1_15_slabs": (2, 20, 6, 5001, 4),
     "V5120_exactly_16_slabs": (2, 20, 6, 5120, 0),
@@ -86,6 +89,14 @@ SHAPES = {
     "V8192_prep_row_8_16_slabs": (2, 10, 5, 8192, 3),
     "V8196_prep_warp_fallback": (2, 10, 5, 8196, 0),
 }
+# two-kernel gradient (U > 32) over several 128-row vocabulary tiles with V % 4 == 0 (MODE 3 Eg / Ef operands):
+# V = 132 (2 tiles, the last of 4 rows), 256 (2 full), 500 (4, the last of 116), 516 (5, the last of 4), crossed with
+# K = U = 49, 73, 151 of dF (3, 4 and 7 stages of 24, the last holding 1, 1 and 7 label positions); 136 frames are
+# three 64-wide dF tiles, the last of 8.  V = 501: the MODE 0 twins (and S on MODE 1 operands).
+for _V in (132, 256, 500, 516, 501):
+    for _U, _stages in ((49, 3), (73, 4), (151, 7)):
+        SHAPES["V%d_U%d_two_kernel_%d_K_stages%s" % (_V, _U, _stages, "_MODE0" if _V % 4 else "")] = \
+            (2, 136, _U, _V, _U % 5)
 
 
 # Shapes whose data need more than the default floors of tests/joint_reference.py, measured on an H100 80GB HBM3:
@@ -102,6 +113,31 @@ FLOORS = {
 @pytest.mark.parametrize("name", list(SHAPES))
 def test_joint_boundary_shape(name):
     check_shape(SHAPES[name], **FLOORS.get(name, {}))
+
+
+def test_plain_joint_long_every_utterance():
+    """The long training shape (N 32, T 500, U 151, V 500: S in one slab of K = 500, dF over K = 151 label positions
+    in 7 stages, dG over K = 500 frames), ragged act_len on every third utterance from the second and label_len on
+    every third from the third.  Every utterance's cost and gradients against smoothed_reference.closed_form at
+    scales (0, 0), the plain joint's fp64 reference in closed form (it never forms [T, U, V]), with the default floors."""
+    import smoothed_reference as sr
+    N, T, U, V, blank = 32, 500, 151, 500, 0
+    rng = np.random.default_rng(67)
+    tl = np.full(N, T, np.int32)
+    ul = np.full(N, U - 1, np.int32)
+    tl[1::3] = rng.integers(T // 2, T, size=len(tl[1::3]))
+    ul[2::3] = rng.integers(0, U - 1, size=len(ul[2::3]))
+    labels = rng.integers(1, V, size=(N, U - 1)).astype(np.int32)
+    trans = (rng.standard_normal((N, T, V)) * 2).astype(np.float32)
+    pred = (rng.standard_normal((N, U, V)) * 2).astype(np.float32)
+    w = np.linspace(0.5, 1.5, N)
+    costs, dF, dG = run_joint(trans, pred, labels, tl, ul, blank, w)
+    c_ref, dF_ref, dG_ref = sr.closed_form(trans, pred, labels, tl, ul, 0.0, 0.0, blank)
+    # cost within 3e-7 relative: measured 1.69e-7 on an H100 80GB HBM3 at 400 W (2.9e-6 when S summed its 500
+    # columns in one accumulator, DESIGN.md §4; 8.3e-8 with the SIMT contractions)
+    rel = np.abs(costs - c_ref) / np.abs(c_ref)
+    assert rel.max() <= 3e-7, rel.max()
+    assert_joint_close(costs, dF, dG, c_ref, dF_ref, dG_ref, labels, tl, ul, blank, scale=w)
 
 
 def test_misaligned_factors_fall_back_and_match():

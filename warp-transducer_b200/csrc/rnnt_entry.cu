@@ -891,8 +891,9 @@ JointWorkspace carve_joint(void* base, int N, int T, int U, int V, bool smooth =
 // ---- tensor-core contractions of the additive joint (rnnt_wgmma.cuh) ---------------------------------
 // N (accumulator columns per CTA) is the smallest instantiated width that holds `n`, tiled beyond 128
 // (a thread holds N/2 accumulators: 128 columns keep two CTAs of 256 threads resident per SM).
-// SMOOTH: the gradient epilogue adds the smoothing terms `sm` (DESIGN.md §9).
-template <int A_MODE, int B_MODE, int KS, bool SMOOTH = false>
+// SMOOTH: the gradient epilogue adds the smoothing terms `sm` (DESIGN.md §9).  STAGEWISE: the stage-wise
+// accumulation of S (rnnt_wgmma.cuh Stagewise), in tiles of at most 64 columns.
+template <int A_MODE, int B_MODE, int KS, bool SMOOTH = false, bool STAGEWISE = false>
 void launch_wgmma(const wg::Operand& A, const wg::Operand& B, int m, int n, int K, int slices, int batch,
                  const wg::Epilogue& epi, cudaStream_t s, int max_tile = 128, const wg::Smooth& sm = wg::Smooth{}) {
     auto go = [&](auto tile) {
@@ -903,6 +904,10 @@ void launch_wgmma(const wg::Operand& A, const wg::Operand& B, int m, int n, int 
             auto kernel = wg::gemm_kernel<A_MODE, B_MODE, NT, KS, wg::Smooth>;
             func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             kernel<<<grid, wg::kThreads, smem, s>>>(A, B, K, slices, epi, sm);
+        } else if constexpr (STAGEWISE) {
+            auto kernel = wg::gemm_kernel<A_MODE, B_MODE, NT, KS, wg::Stagewise>;
+            func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            kernel<<<grid, wg::kThreads, smem, s>>>(A, B, K, slices, epi, wg::Stagewise{});
         } else {
             auto kernel = wg::gemm_kernel<A_MODE, B_MODE, NT, KS>;
             func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -910,8 +915,8 @@ void launch_wgmma(const wg::Operand& A, const wg::Operand& B, int m, int n, int 
         }
     };
     if (n <= 32) go(std::integral_constant<int, 32>{});
-    else if (n <= 64 || max_tile <= 64) go(std::integral_constant<int, 64>{});
-    else go(std::integral_constant<int, 128>{});
+    else if (STAGEWISE || n <= 64 || max_tile <= 64) go(std::integral_constant<int, 64>{});
+    else if constexpr (!STAGEWISE) go(std::integral_constant<int, 128>{});
 }
 
 // t.acts / t.grads: the transcription factor f [N,T,V] and its gradient; g / dG: the prediction factor
@@ -986,10 +991,16 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
             // float4 operand fetches when every row of Ef / Eg starts on a 16-byte boundary
             // partial sums of slice ks land in slab ks: part[ks][b][t][u]
             const wg::Epilogue epi{nullptr, 0, 0, 0, w.part, (long long)d.rows, (long long)T * U, U, 1};
-            if (V % 4 == 0)
-                launch_wgmma<2, 2, 32>(A, B, T, U, V, slices, N, epi, s);
-            else
-                launch_wgmma<1, 1, 32>(A, B, T, U, V, slices, N, epi, s);
+            // slabs of more than 8 stages (256 columns) accumulate stage-wise: one accumulator would take more
+            // than 96 MMAs, each truncating toward zero (rnnt_wgmma.cuh Stagewise)
+            const bool stagewise = (V + slices - 1) / slices > 256;
+            if (V % 4 == 0) {
+                if (stagewise) launch_wgmma<2, 2, 32, false, true>(A, B, T, U, V, slices, N, epi, s);
+                else launch_wgmma<2, 2, 32>(A, B, T, U, V, slices, N, epi, s);
+            } else {
+                if (stagewise) launch_wgmma<1, 1, 32, false, true>(A, B, T, U, V, slices, N, epi, s);
+                else launch_wgmma<1, 1, 32>(A, B, T, U, V, slices, N, epi, s);
+            }
         } else {
             Operand A{w.ef, (size_t)T * V, V, 1}, B{w.eg, (size_t)U * V, V, 1};
             dim3 grid((U + 63) / 64, (T + 63) / 64, N * slices);

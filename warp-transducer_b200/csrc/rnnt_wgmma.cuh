@@ -12,7 +12,9 @@
 // fp32 accuracy on tf32 tensor cores: every operand element x is split by the producer threads into
 // hi = tf32(x) (truncated) and lo = x - hi (exact in fp32; the tensor core keeps its top 11 bits), and
 // each k-step issues three MMAs into the same accumulator: hi*hi + hi*lo + lo*hi.  The dropped lo*lo
-// term is 2^-20 relative; the sums feed a logarithm (S) and gradients checked to 1e-4 (P, Q).
+// term is 2^-20 relative; the sums feed a logarithm (S) and gradients checked to 1e-4 (P, Q).  The tensor
+// core's accumulation rounds toward zero, up to an ulp per MMA in one direction: S, whose bias every lattice
+// cell sees, therefore accumulates stage-wise (Stagewise below); P and Q keep one accumulator.
 //
 // Operands are staged global -> registers (split) -> shared memory in the canonical K-major NO-SWIZZLE
 // ("interleave") layout of the wgmma matrix descriptor (tf32 operands must be K-major), in units of
@@ -393,11 +395,22 @@ __device__ __forceinline__ float smooth_acc(float acc, const Smooth& sm, int b, 
     acc += cf.x;
     return sm.w ? fmaf(cf.y, __ldg(sm.w + m), acc) : acc;
 }
+// Stage-wise accumulation (gemm_kernel's trailing parameter, the S contraction): the tensor core accumulates in fp32
+// rounding toward zero, so with all-positive terms every MMA into an accumulator loses up to an ulp of the running
+// sum, in the same direction - 189 MMAs over K = 500 made S ~1.5e-5 too small.  Stagewise restarts the accumulator
+// every k-stage, issues the stage's hi*lo and lo*hi MMAs before its hi*hi ones (while the running sum is ~2^-10 of
+// the stage's, their truncations are that much smaller), and adds the stage into an fp32 register total with
+// round-to-nearest: KS / 8 biased roundings per stage instead of 3 KS / 8 per stage for the whole slab.
+struct Stagewise {};
+template <typename... Sm> struct IsStagewise : std::false_type {};
+template <> struct IsStagewise<Stagewise> : std::true_type {};
+
 // gemm_kernel's form: the smoothing terms come as an optional trailing parameter (none: the plain epilogue)
 __device__ __forceinline__ float smooth_acc_opt(float acc, int, int, int) { return acc; }
 __device__ __forceinline__ float smooth_acc_opt(float acc, int b, int m, int n, const Smooth& sm) {
     return smooth_acc<true>(acc, sm, b, m, n);
 }
+__device__ __forceinline__ float smooth_acc_opt(float acc, int, int, int, const Stagewise&) { return acc; }
 
 // Accumulator fragment of this thread (see Mma): row and column of element i relative to the warpgroup's tile
 __device__ __forceinline__ constexpr int frag_row(int i) { return 8 * ((i >> 1) & 1); }
@@ -408,12 +421,15 @@ __device__ __forceinline__ constexpr int frag_col(int i) { return 8 * (i >> 2) +
 // One shared-memory stage buffer per CTA: the footprint stays small, so several CTAs are resident per SM
 // and cover each other's load -> split -> multiply chains; within a CTA the global loads of stage s+1 are in
 // flight in registers while stage s is multiplied.  Elements with m >= A.mn_valid or n >= B.mn_valid are skipped.
-// Sm: empty (the plain kernel, named gemm_kernel<A_MODE, B_MODE, N, KS>) or one Smooth, whose terms the epilogue
-// adds (the smoothed joint's dF / dG, DESIGN.md §9).
+// Sm: empty (the plain kernel, named gemm_kernel<A_MODE, B_MODE, N, KS>), one Smooth, whose terms the epilogue
+// adds (the smoothed joint's dF / dG, DESIGN.md §9), or Stagewise (S: the accumulation above; its register total
+// needs N / 2 more registers per thread, so at most 64 columns, and two CTAs per SM at 64).
 template <int A_MODE, int B_MODE, int N, int KS, typename... Sm>
-__global__ void __launch_bounds__(kThreads, N <= 64 ? 3 : 2)
+__global__ void __launch_bounds__(kThreads, N <= 32 || (N <= 64 && !IsStagewise<Sm...>::value) ? 3 : 2)
 gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue epi, Sm... sm) {
     static_assert(sizeof...(Sm) <= 1, "at most one set of smoothing terms");
+    constexpr bool STAGEWISE = IsStagewise<Sm...>::value;
+    static_assert(!STAGEWISE || N <= 64, "the stage-wise total fits the register budget up to 64 columns");
     static_assert(N % 32 == 0 && N >= 32 && N <= 128 && KS % 8 == 0, "wgmma shape");
     constexpr uint32_t A_BYTES = TileGeom::bytes(128, KS), B_BYTES = TileGeom::bytes(N, KS);
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -437,8 +453,11 @@ gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue 
         rb.load(kbeg, kend);
     }
     float acc[N / 2];
+    float total[STAGEWISE ? N / 2 : 1];
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
+#pragma unroll
+    for (int i = 0; i < (STAGEWISE ? N / 2 : 1); ++i) total[i] = 0.0f;
     // this warpgroup's 64 rows of A start 8 row groups into the tile
     const uint32_t a_off = (uint32_t)group * 8 * TileGeom::sbo(KS);
 
@@ -459,12 +478,29 @@ gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue 
             const uint64_t al = smem_desc(s32(a_lo) + a_off + TileGeom::kstep(j), TileGeom::lbo(), TileGeom::sbo(KS));
             const uint64_t bh = smem_desc(s32(b_hi) + TileGeom::kstep(j), TileGeom::lbo(), TileGeom::sbo(KS));
             const uint64_t bl = smem_desc(s32(b_lo) + TileGeom::kstep(j), TileGeom::lbo(), TileGeom::sbo(KS));
-            Mma<N>::run(acc, ah, bh, 1);
-            Mma<N>::run(acc, ah, bl, 1);
-            Mma<N>::run(acc, al, bh, 1);
+            if (STAGEWISE) {   // the stage's small products first, the first of them overwriting the accumulator
+                Mma<N>::run(acc, ah, bl, j != 0);
+                Mma<N>::run(acc, al, bh, 1);
+            } else {
+                Mma<N>::run(acc, ah, bh, 1);
+                Mma<N>::run(acc, ah, bl, 1);
+                Mma<N>::run(acc, al, bh, 1);
+            }
+        }
+        if (STAGEWISE) {
+#pragma unroll
+            for (int j = 0; j < KS / 8; ++j) {
+                const uint64_t ah = smem_desc(s32(a_hi) + a_off + TileGeom::kstep(j), TileGeom::lbo(), TileGeom::sbo(KS));
+                const uint64_t bh = smem_desc(s32(b_hi) + TileGeom::kstep(j), TileGeom::lbo(), TileGeom::sbo(KS));
+                Mma<N>::run(acc, ah, bh, 1);
+            }
         }
         mma_commit();
         mma_wait_all();
+        if (STAGEWISE) {
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) total[i] += acc[i];
+        }
     }
 
     // epilogue: element i of the fragment is (row m_base + frag_row(i), column n_base + frag_col(i))
@@ -477,7 +513,7 @@ gemm_kernel(const Operand A, const Operand B, int K, int slices, const Epilogue 
     for (int i = 0; i < N / 2; ++i) {
         const int m = m_base + frag_row(i), n = n_base + frag_col(i);
         if (m < A.mn_valid && n < B.mn_valid) {
-            const float x = smooth_acc_opt(acc[i], b, m, n, sm...);
+            const float x = smooth_acc_opt(STAGEWISE ? total[STAGEWISE ? i : 0] : acc[i], b, m, n, sm...);
             op[m * epi.out_m + n * epi.out_n] = ip ? x * __ldg(ip + (m * epi.in_m + n * epi.in_n)) : x;
         }
     }
