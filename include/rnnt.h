@@ -406,6 +406,87 @@ rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const in
                                               int s_range, int* ranges, const void* workspace,
                                               struct rnntOptions options);
 
+/*
+ * Lattice options, passed BY VALUE to the *_lat entries below.  Unlike rnntGradOptions they change the lattice, so
+ * they change the cost as well as the gradient.  Zero-initialised = off, and the *_lat entries then launch exactly
+ * the kernels of the entries without them and compute the same results, bitwise.
+ *
+ *   delay_penalty  lambda of the delay-penalised transducer (Kang et al., "Delay-penalized transducer for
+ *                  low-latency streaming ASR", ICASSP 2023; k2's delay_penalty).  With T_b the frame count of
+ *                  utterance b after the usual clamp into [1, maxT], every valid cell (t, u) with a label
+ *                  transition (u < U_b - 1) gets
+ *                      lp_y(t,u) <- lp_y(t,u) + lambda ((T_b - 1)/2 - t)
+ *                  and nothing else changes: blank factors are unchanged, the cost is -log of the sum over all paths
+ *                  of the penalised factors (so it includes the penalty and can be negative), and the gradient is the
+ *                  exact gradient of that cost.  A path's log-score gains lambda sum_labels ((T_b - 1)/2 - t_emit),
+ *                  which favours emitting labels early.  Pruned loss: the same rule on the covered cells; uncovered
+ *                  cells stay log zero.  Additive joint: the penalty is added after the smoothing interpolation.
+ *                  With FastEmit, the surrogate stays -fastemit_lambda sum sg[e_y] log p_y, with e_y the label
+ *                  occupancy of the penalised lattice and p_y the unpenalised softmax probability; clamp is unchanged.
+ *                  Must be finite and >= 0 (a negative value is rejected, where k2 ignores it); 0 = off.
+ * Invalid values return RNNT_STATUS_INVALID_VALUE before any device access.  Workspace sizes do not change.
+ */
+struct rnntLatticeOptions {
+    float delay_penalty;   /* float for every storage type, as rnntGradOptions */
+};
+#ifndef __cplusplus
+typedef struct rnntLatticeOptions rnntLatticeOptions;
+#endif
+
+/* rnnt_b200_loss_async_ex with lattice options (dtype, layout, costs, grad_scale and gradient options as there). */
+rnntStatus_t rnnt_b200_loss_async_lat(int dtype, int layout, const void* activations, void* gradients,
+                                      const int* flat_labels, const int* label_lengths,
+                                      const int* input_lengths, int alphabet_size, int minibatch,
+                                      void* costs_device, double grad_scale, struct rnntGradOptions grad_options,
+                                      struct rnntLatticeOptions lattice_options, void* workspace,
+                                      struct rnntOptions options);
+/* Training-step split of the same for all four storage types (costs_device / grad_costs_device are double* for
+ * fp64, float* otherwise).  The backward half's pass over the logits needs the penalty again: it must get the
+ * lattice options its forward got, as it must get the same workspace. */
+rnntStatus_t rnnt_b200_forward_lat(int dtype, const void* activations, const int* flat_labels,
+                                   const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                   int minibatch, void* costs_device, int prepare_backward,
+                                   struct rnntLatticeOptions lattice_options, void* workspace,
+                                   struct rnntOptions options);
+rnntStatus_t rnnt_b200_backward_lat(int dtype, const void* activations, void* gradients,
+                                    const int* flat_labels, const int* label_lengths,
+                                    const int* input_lengths, int alphabet_size, int minibatch,
+                                    const void* grad_costs_device, double grad_scale,
+                                    struct rnntGradOptions grad_options, struct rnntLatticeOptions lattice_options,
+                                    void* workspace, struct rnntOptions options);
+/* The pruned loss with lattice options: rnnt_b200_pruned_loss_async_ex, _forward and _backward_ex plus
+ * lattice_options; the backward half must get the options (and the ranges) its forward got. */
+rnntStatus_t rnnt_b200_pruned_loss_async_lat(int dtype, int layout, const void* activations, void* gradients,
+                                             const int* ranges, int s_range, const int* flat_labels,
+                                             const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                             int minibatch, void* costs_device, double grad_scale,
+                                             struct rnntGradOptions grad_options,
+                                             struct rnntLatticeOptions lattice_options, void* workspace,
+                                             struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_forward_lat(int dtype, const void* activations, const int* ranges, int s_range,
+                                          const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                          int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
+                                          struct rnntLatticeOptions lattice_options, void* workspace,
+                                          struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_backward_lat(int dtype, const void* activations, void* gradients, const int* ranges,
+                                           int s_range, const int* flat_labels, const int* label_lengths,
+                                           const int* input_lengths, int alphabet_size, int minibatch,
+                                           const void* grad_costs_device, double grad_scale,
+                                           struct rnntGradOptions grad_options,
+                                           struct rnntLatticeOptions lattice_options, void* workspace,
+                                           struct rnntOptions options);
+/* The additive joint's forward half with smoothing (rnntSmoothOptions, both 0 = the plain joint, which then wants
+ * rnnt_b200_add_joint_workspace_size; else rnnt_b200_add_joint_smoothed_workspace_size) and lattice options.  The
+ * penalty lives in the factors this forward leaves in the workspace, so the backward halves
+ * (rnnt_b200_add_joint_backward, _backward_ex, _smoothed_backward, with the smoothing scales of the forward) take no
+ * lattice options, and rnnt_b200_add_joint_prune_ranges gives the windows of the penalised lattice. */
+rnntStatus_t rnnt_b200_add_joint_forward_lat(const float* trans, const float* pred, const int* flat_labels,
+                                             const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                             int minibatch, float* costs_device, int prepare_backward,
+                                             struct rnntSmoothOptions smooth,
+                                             struct rnntLatticeOptions lattice_options, void* workspace,
+                                             struct rnntOptions options);
+
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug
  * builds (include/detail/cpu_rnnt.h:167-170); tests/test_gpu_round2.py does the same.  Synchronises. */

@@ -110,21 +110,20 @@ __device__ __forceinline__ void chunk_issue(const T* __restrict__ acts, T* tile,
 // The element walk is group-parallel: TPR lanes per row, results handed over through shared memory.
 // The CTA size NT is a template parameter (tuning hook RNNT_B200_CHUNK_NT; default 256).
 // =================================================================================================
-template <typename T, int TPR, int NT, bool PRUNED>
-__global__ void __launch_bounds__(NT)
-rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels, const int* __restrict__ xlen,
-                      const int* __restrict__ ylen, typename Real<T>::pair* __restrict__ stat,
-                      typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor, const uint32_t wait_ns,
-                      const Prune p) {
+template <typename T, int TPR, int NT, bool PRUNED, bool DELAY>
+__device__ __forceinline__ void rowstats_chunk(const T* __restrict__ acts, const int* __restrict__ labels,
+                                               const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                               typename Real<T>::pair* __restrict__ stat,
+                                               typename Lat<T>::fac* __restrict__ lp2, const Dims& d,
+                                               const int hmajor, const uint32_t wait_ns, const Prune& p,
+                                               const T delay, unsigned char* chunk_raw,
+                                               unsigned long long* bar_store, typename Real<T>::pair* row_ms) {
     using R = Real<T>;
     using Pair = typename R::pair;
     constexpr int ROWS = NT / TPR;
     static_assert(TPR <= 32 && NT % 32 == 0, "the lanes of a row sit in one warp");
-    extern __shared__ __align__(128) unsigned char chunk_raw[];
     T* tile = reinterpret_cast<T*>(chunk_raw);
-    __shared__ __align__(8) unsigned long long bar_store;
-    __shared__ Pair row_ms[ROWS];   // (max, sum of exponentials) per row, group leaders -> row owners
-    const uint32_t bar = smem_u32(&bar_store);
+    const uint32_t bar = smem_u32(bar_store);
     const uint32_t r0 = blockIdx.x * ROWS;
     const uint32_t nrows = min((uint32_t)ROWS, d.rows - r0);
     const int V = d.V;
@@ -137,6 +136,7 @@ rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels
     bool valid = threadIdx.x < nrows;
     int y = -1;
     size_t q = 0;
+    T pen = T(0);   // DELAY: the row's label penalty
     if (valid) {
         uint32_t u, b, t;
         int Tb, Ub;
@@ -145,6 +145,7 @@ rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels
         valid = !row_padding<PRUNED>(t, u, Tb, Ub);
         if (valid && (int)u < Ub - 1) y = __ldg(labels + (size_t)b * (d.maxU - 1) + u);
         q = skew(d, b, t, u);
+        if constexpr (DELAY) pen = delay * delay_bracket<T>(Tb, t);
     }
     // one barrier: publishes the mbarrier to the waiters and tells whether any row of the chunk is a
     // real cell (a fully padded chunk - ragged batches only - costs one wasted read, nothing else)
@@ -213,8 +214,39 @@ rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels
         st.x = M;
         st.y = lse;
         stat[r0 + threadIdx.x] = st;
-        lp2[q] = Lat<T>::make((x[d.blank] - M) - lse, y >= 0 ? (x[y] - M) - lse : T(0), y >= 0);
+        if constexpr (DELAY)
+            lp2[q] = Lat<T>::make((x[d.blank] - M) - lse, y >= 0 ? (x[y] - M) - lse + pen : T(0), y >= 0);
+        else
+            lp2[q] = Lat<T>::make((x[d.blank] - M) - lse, y >= 0 ? (x[y] - M) - lse : T(0), y >= 0);
     }
+}
+template <typename T, int TPR, int NT, bool PRUNED>
+__global__ void __launch_bounds__(NT)
+rowstats_chunk_kernel(const T* __restrict__ acts, const int* __restrict__ labels, const int* __restrict__ xlen,
+                      const int* __restrict__ ylen, typename Real<T>::pair* __restrict__ stat,
+                      typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor, const uint32_t wait_ns,
+                      const Prune p) {
+    // shared memory: declared here, not in the body (in a device function the dynamic part would take the
+    // 1024-byte alignment of the tensor-core kernels' and start elsewhere)
+    extern __shared__ __align__(128) unsigned char chunk_raw[];
+    __shared__ __align__(8) unsigned long long bar_store;
+    __shared__ typename Real<T>::pair row_ms[NT / TPR];   // (max, sum of exponentials) per row, group leaders -> row owners
+    rowstats_chunk<T, TPR, NT, PRUNED, false>(acts, labels, xlen, ylen, stat, lp2, d, hmajor, wait_ns, p, T(0), chunk_raw,
+                                              &bar_store, row_ms);
+}
+template <typename T, int TPR, int NT, bool PRUNED>
+__global__ void __launch_bounds__(NT)
+rowstats_chunk_delay_kernel(const T* __restrict__ acts, const int* __restrict__ labels, const int* __restrict__ xlen,
+                            const int* __restrict__ ylen, typename Real<T>::pair* __restrict__ stat,
+                            typename Lat<T>::fac* __restrict__ lp2, const Dims d, const int hmajor,
+                            const uint32_t wait_ns, const Prune p, const T delay) {
+    // shared memory: declared here, not in the body (in a device function the dynamic part would take the
+    // 1024-byte alignment of the tensor-core kernels' and start elsewhere)
+    extern __shared__ __align__(128) unsigned char chunk_raw[];
+    __shared__ __align__(8) unsigned long long bar_store;
+    __shared__ typename Real<T>::pair row_ms[NT / TPR];   // (max, sum of exponentials) per row, group leaders -> row owners
+    rowstats_chunk<T, TPR, NT, PRUNED, true>(acts, labels, xlen, ylen, stat, lp2, d, hmajor, wait_ns, p, delay, chunk_raw,
+                                             &bar_store, row_ms);
 }
 
 // =================================================================================================
@@ -231,22 +263,24 @@ template <typename T> struct ChunkRow {
     int valid;
 };
 
-template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED>
-__global__ void __launch_bounds__(NT)
-grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
-                  const int* __restrict__ xlen, const int* __restrict__ ylen,
-                  const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                  const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
-                  const T scale_in, const T* __restrict__ scale_vec, const Dims d, const int hmajor,
-                  const uint32_t wait_ns, const GradReg<T> reg, const Prune p) {
+template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED, bool DELAY>
+__device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __restrict__ grads,
+                                           const int* __restrict__ labels, const int* __restrict__ xlen,
+                                           const int* __restrict__ ylen,
+                                           const typename Real<T>::pair* __restrict__ stat,
+                                           const typename Lat<T>::val* __restrict__ alphas,
+                                           const typename Lat<T>::val* __restrict__ betas,
+                                           const typename Lat<T>::val* __restrict__ llf, const T scale_in,
+                                           const T* __restrict__ scale_vec, const Dims d, const int hmajor,
+                                           const uint32_t wait_ns, const GradReg<T> reg, const Prune p,
+                                           const T delay_log2, unsigned char* chunk_raw,
+                                           unsigned long long* bar_store) {
     using R = Real<T>;
     using Pair = typename R::pair;
     constexpr int ROWS = NT / TPR;
-    extern __shared__ __align__(128) unsigned char chunk_raw[];
     T* tile = reinterpret_cast<T*>(chunk_raw);
-    __shared__ __align__(8) unsigned long long bar_store;
     const ChunkMap<TPR> map(hmajor);
-    const uint32_t bar = smem_u32(&bar_store);
+    const uint32_t bar = smem_u32(bar_store);
     // chunks in reverse order: the tail of pass 1 is met first in L2
     const uint32_t nchunks = gridDim.x;
     const uint32_t r0 = (nchunks - 1 - blockIdx.x) * ROWS;
@@ -294,6 +328,7 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
         if constexpr (REG) {
             if (v) fastemit_fold(rg, reg, b, t, u, d);
         }
+        if constexpr (DELAY) delay_fold(rg, delay_log2, Tb, t);
         c.m = rg.m, c.cA = rg.cA, c.cB = rg.cB, c.cL = rg.cL, c.y = rg.y;
         c.valid = v ? 1 : (inrange ? 0 : -1);   // -1: row does not exist (past the end of the tensor)
         return c;
@@ -392,6 +427,35 @@ grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* 
         __syncthreads();
         for (uint32_t k = threadIdx.x; k < nelem; k += NT) gout[k] = tile[k];
     }
+}
+template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED>
+__global__ void __launch_bounds__(NT)
+grad_chunk_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
+                  const int* __restrict__ xlen, const int* __restrict__ ylen,
+                  const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                  const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                  const T scale_in, const T* __restrict__ scale_vec, const Dims d, const int hmajor,
+                  const uint32_t wait_ns, const GradReg<T> reg, const Prune p) {
+    extern __shared__ __align__(128) unsigned char chunk_raw[];   // declared here: see rowstats_chunk_kernel
+    __shared__ __align__(8) unsigned long long bar_store;
+    grad_chunk<T, TPR, NT, SCALED, REG, PRUNED, false>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                       scale_in, scale_vec, d, hmajor, wait_ns, reg, p, T(0), chunk_raw,
+                                                       &bar_store);
+}
+template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED>
+__global__ void __launch_bounds__(NT)
+grad_chunk_delay_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
+                        const int* __restrict__ xlen, const int* __restrict__ ylen,
+                        const typename Real<T>::pair* __restrict__ stat,
+                        const typename Lat<T>::val* __restrict__ alphas, const typename Lat<T>::val* __restrict__ betas,
+                        const typename Lat<T>::val* __restrict__ llf, const T scale_in,
+                        const T* __restrict__ scale_vec, const Dims d, const int hmajor, const uint32_t wait_ns,
+                        const GradReg<T> reg, const Prune p, const T delay_log2) {
+    extern __shared__ __align__(128) unsigned char chunk_raw[];   // declared here: see rowstats_chunk_kernel
+    __shared__ __align__(8) unsigned long long bar_store;
+    grad_chunk<T, TPR, NT, SCALED, REG, PRUNED, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                      scale_in, scale_vec, d, hmajor, wait_ns, reg, p, delay_log2,
+                                                      chunk_raw, &bar_store);
 }
 
 }  // namespace b200rnnt

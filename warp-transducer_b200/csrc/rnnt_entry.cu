@@ -276,6 +276,11 @@ inline bool smooth_valid(const rnntSmoothOptions& o) {
     return std::isfinite(l) && std::isfinite(a) && l >= 0.0 && a >= 0.0 && l + a <= 1.0 + 0x1p-23;
 }
 inline bool smooth_on(const rnntSmoothOptions& o) { return o.lm_only_scale != 0.0f || o.am_only_scale != 0.0f; }
+// lattice options (include/rnnt.h rnntLatticeOptions): the delay penalty (DESIGN.md §10)
+inline bool lattice_valid(const rnntLatticeOptions& o) {
+    return std::isfinite(o.delay_penalty) && o.delay_penalty >= 0.0f;
+}
+inline bool delay_on(const rnntLatticeOptions& o) { return o.delay_penalty > 0.0f; }
 template <typename T> GradReg<T> make_grad_reg(const rnntGradOptions& o, const Workspace& w) {
     GradReg<T> r;
     r.lp2 = static_cast<const typename Lat<T>::fac*>(w.lp2);
@@ -302,6 +307,7 @@ struct Call {
     rnntGradOptions grad;
     bool pruned = false;     // logits [N,maxT,R,V] over the windows Tensors::ranges (DESIGN.md §8)
     rnntSmoothOptions smooth = {0.0f, 0.0f};   // additive joint: lm-only / am-only scales (DESIGN.md §9)
+    rnntLatticeOptions lattice = {0.0f};       // delay penalty of the label factors (DESIGN.md §10)
 };
 Call full_call(double scale, bool async = true, bool tunv = false, rnntGradOptions grad = {0.0f, 0.0f}) {
     return Call{kFull, async, false, tunv, scale, nullptr, grad};
@@ -330,7 +336,8 @@ struct Tensors {
 // The checks of every compute call, all before any device access; the first that fails decides the status.
 rnntStatus_t check_call(const Tensors& t, const Call& c) {
     const rnntOptions& opt = t.opt;
-    if (!grad_options_valid(c.grad) || !smooth_valid(c.smooth)) return RNNT_STATUS_INVALID_VALUE;
+    if (!grad_options_valid(c.grad) || !smooth_valid(c.smooth) || !lattice_valid(c.lattice))
+        return RNNT_STATUS_INVALID_VALUE;
     if (!t.acts || !t.labels || !t.ylen || !t.xlen || (!t.costs && c.phase != kBackward) || !t.workspace ||
         t.V <= 0 || t.N <= 0 || opt.maxT <= 0 || opt.maxU <= 0 || (c.phase == kBackward && !t.grads))
         return RNNT_STATUS_INVALID_VALUE;  // reference src/rnnt_entrypoint.cpp:49-59
@@ -384,6 +391,9 @@ struct Group {
     bool pdl;            // launch the dependent kernels with programmatic stream serialization
     bool pruned;         // the PRUNED streaming kernels, given `pr` (the dense ones get ranges == NULL)
     Prune pr;
+    bool delay;          // delay penalty on: the *_delay_kernel twins, given `pen` (pass 1) and `pen_log2` (pass 2)
+    T pen;               // lambda
+    T pen_log2;          // lambda log2(e)
     bool scaled() const { return scale != T(1) || scale_vec; }
 };
 
@@ -402,18 +412,27 @@ template <typename F, typename... Flags> void with_flags(F&& f, bool first, Flag
 template <typename T, int VEC, int NV, typename IO>
 void launch_row(const Group<T, IO>& g, int pass) {
     using Val = const typename Lat<T>::val*;
-    with_flags([&](auto scaled, auto reg, auto pruned) {
+    with_flags([&](auto scaled, auto reg, auto pruned, auto delay) {
         constexpr bool SCALED = decltype(scaled)::value, REG = decltype(reg)::value, PRUNED = decltype(pruned)::value;
-        if (pass == 1)
-            rowstats_row_kernel<T, VEC, NV, IO, PRUNED><<<g.d.rows, RowThreads<IO>::value, 0, g.s>>>(
-                g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
-                static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d, g.pr);
+        constexpr bool DELAY = decltype(delay)::value;
+        auto* stat = static_cast<typename Real<T>::pair*>(g.w.stat);
+        auto* lp2 = static_cast<typename Lat<T>::fac*>(g.w.lp2);
+        const dim3 grid(g.d.rows), block(RowThreads<IO>::value);
+        if (pass == 1 && DELAY)
+            rowstats_row_delay_kernel<T, VEC, NV, IO, PRUNED><<<grid, block, 0, g.s>>>(
+                g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, g.pr, g.pen);
+        else if (pass == 1)
+            rowstats_row_kernel<T, VEC, NV, IO, PRUNED><<<grid, block, 0, g.s>>>(
+                g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, g.pr);
+        else if (DELAY)
+            launch_k(grad_row_delay_kernel<T, VEC, NV, SCALED, IO, REG, PRUNED>, grid, block, 0, g.s, g.pdl, g.acts,
+                     g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas), static_cast<Val>(g.w.betas),
+                     static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr, g.pen_log2);
         else
-            launch_k(grad_row_kernel<T, VEC, NV, SCALED, IO, REG, PRUNED>, dim3(g.d.rows), dim3(RowThreads<IO>::value),
-                     0, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen,
-                     static_cast<const typename Real<T>::pair*>(g.w.stat), static_cast<Val>(g.w.alphas),
-                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
-    }, g.scaled(), g.reg, g.pruned);
+            launch_k(grad_row_kernel<T, VEC, NV, SCALED, IO, REG, PRUNED>, grid, block, 0, g.s, g.pdl, g.acts,
+                     g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas), static_cast<Val>(g.w.betas),
+                     static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
+    }, g.scaled(), g.reg, g.pruned, g.delay);
     ++g_last_launches;
 }
 
@@ -422,18 +441,27 @@ void launch_tile(const Group<T, IO>& g, int pass) {
     using Val = const typename Lat<T>::val*;
     const uint64_t warps = ((uint64_t)g.d.rows * LPR + 31) / 32;
     const unsigned grid = (unsigned)((warps + 7) / 8);
-    with_flags([&](auto scaled, auto reg, auto pruned) {
+    with_flags([&](auto scaled, auto reg, auto pruned, auto delay) {
         constexpr bool SCALED = decltype(scaled)::value, REG = decltype(reg)::value, PRUNED = decltype(pruned)::value;
-        if (pass == 1)
+        constexpr bool DELAY = decltype(delay)::value;
+        auto* stat = static_cast<typename Real<T>::pair*>(g.w.stat);
+        auto* lp2 = static_cast<typename Lat<T>::fac*>(g.w.lp2);
+        if (pass == 1 && DELAY)
+            rowstats_tile_delay_kernel<T, VEC, LPR, IO, PRUNED><<<grid, 256, 0, g.s>>>(
+                g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, g.pr, g.pen);
+        else if (pass == 1)
             rowstats_tile_kernel<T, VEC, LPR, IO, PRUNED><<<grid, 256, 0, g.s>>>(
-                g.acts, g.labels, g.xlen, g.ylen, static_cast<typename Real<T>::pair*>(g.w.stat),
-                static_cast<typename Lat<T>::fac*>(g.w.lp2), g.d, g.pr);
+                g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, g.pr);
+        else if (DELAY)
+            launch_k(grad_tile_delay_kernel<T, VEC, LPR, SCALED, IO, REG, PRUNED>, dim3(grid), dim3(256), 0, g.s,
+                     g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas),
+                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr,
+                     g.pen_log2);
         else
             launch_k(grad_tile_kernel<T, VEC, LPR, SCALED, IO, REG, PRUNED>, dim3(grid), dim3(256), 0, g.s, g.pdl,
-                     g.acts, g.grads, g.labels, g.xlen, g.ylen, static_cast<const typename Real<T>::pair*>(g.w.stat),
-                     static_cast<Val>(g.w.alphas), static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale,
-                     g.scale_vec, g.d, g.gr, g.pr);
-    }, g.scaled(), g.reg, g.pruned);
+                     g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas),
+                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr);
+    }, g.scaled(), g.reg, g.pruned, g.delay);
     ++g_last_launches;
 }
 
@@ -546,19 +574,28 @@ bool chunk_pass(const Group<T, T>& g, int pass) {
     auto go = [&](auto tpr_c, auto nt_c) {
         constexpr int TPR = decltype(tpr_c)::value, NT = decltype(nt_c)::value;
         if constexpr (NT / TPR >= 4) {
-            with_flags([&](auto scaled, auto reg, auto pruned) {
+            with_flags([&](auto scaled, auto reg, auto pruned, auto delay) {
                 constexpr bool SCALED = decltype(scaled)::value, REG = decltype(reg)::value;
-                constexpr bool PRUNED = decltype(pruned)::value;
-                if (pass == 1)
+                constexpr bool PRUNED = decltype(pruned)::value, DELAY = decltype(delay)::value;
+                Pair* stat = static_cast<Pair*>(g.w.stat);
+                Fac* lp2 = static_cast<Fac*>(g.w.lp2);
+                const Val *al = static_cast<const Val*>(g.w.alphas), *be = static_cast<const Val*>(g.w.betas);
+                const Val* llf = static_cast<const Val*>(g.w.llf);
+                if (pass == 1 && DELAY)
+                    prefer_smem(rowstats_chunk_delay_kernel<T, TPR, NT, PRUNED>)<<<grid, NT, smem, g.s>>>(
+                        g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, hmajor, wait_ns, g.pr, g.pen);
+                else if (pass == 1)
                     prefer_smem(rowstats_chunk_kernel<T, TPR, NT, PRUNED>)<<<grid, NT, smem, g.s>>>(
-                        g.acts, g.labels, g.xlen, g.ylen, static_cast<Pair*>(g.w.stat), static_cast<Fac*>(g.w.lp2), g.d,
-                        hmajor, wait_ns, g.pr);
+                        g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, hmajor, wait_ns, g.pr);
+                else if (DELAY)
+                    launch_k(prefer_smem(grad_chunk_delay_kernel<T, TPR, NT, SCALED, REG, PRUNED>), dim3(grid), dim3(NT),
+                             smem, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, al, be, llf, g.scale,
+                             g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr, g.pen_log2);
                 else
                     launch_k(prefer_smem(grad_chunk_kernel<T, TPR, NT, SCALED, REG, PRUNED>), dim3(grid), dim3(NT), smem,
-                             g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, static_cast<const Pair*>(g.w.stat),
-                             static_cast<const Val*>(g.w.alphas), static_cast<const Val*>(g.w.betas),
-                             static_cast<const Val*>(g.w.llf), g.scale, g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr);
-            }, g.scaled(), g.reg, g.pruned);
+                             g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, al, be, llf, g.scale,
+                             g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr);
+            }, g.scaled(), g.reg, g.pruned, g.delay);
         }
     };
     auto with_rpt = [&](auto tpr_c) {
@@ -725,6 +762,9 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
         g.pdl = pdl;
         g.pruned = c.pruned;
         g.pr = Prune{c.pruned ? t.ranges + (size_t)b0 * opt.maxT : nullptr, FastDiv((uint32_t)rows_u)};
+        g.delay = delay_on(c.lattice);
+        g.pen = (T)c.lattice.delay_penalty;
+        g.pen_log2 = (T)((double)c.lattice.delay_penalty * 1.4426950408889634);
         return g;
     };
     const bool with_beta = grads || c.want_beta;
@@ -1013,13 +1053,28 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
                     A, B, T, U, V, slices, EpiPartial{w.part, (size_t)d.rows, T, U, slices});
             }
         }
+        // the delay penalty (DESIGN.md §10) goes into the factors here; every later kernel reads them from lp2
+        const bool dl = delay_on(c.lattice);
+        const unsigned sgrid = (d.rows + 255) / 256;
         if (!sm) {
-            EpiStats<> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d};
-            joint_stats_kernel<<<(d.rows + 255) / 256, 256, 0, s>>>(w.part, slices, epi);
+            if (!dl) {
+                EpiStats<> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d};
+                joint_stats_kernel<<<sgrid, 256, 0, s>>>(w.part, slices, epi);
+            } else {
+                EpiStats<false, true> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d};
+                epi.delay = c.lattice.delay_penalty;
+                joint_stats_delay_kernel<<<sgrid, 256, 0, s>>>(w.part, slices, epi);
+            }
         } else {
-            EpiStats<true> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d, w.sg, w.A, w.lug,
-                               cfull, lml, lma};
-            joint_stats_kernel<true><<<(d.rows + 255) / 256, 256, 0, s>>>(w.part, slices, epi);
+            if (!dl) {
+                EpiStats<true> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d, w.sg, w.A, w.lug,
+                                   cfull, lml, lma};
+                joint_stats_kernel<true><<<sgrid, 256, 0, s>>>(w.part, slices, epi);
+            } else {
+                EpiStats<true, true> epi{f, g, w.mf, w.mg, labels, xlen, ylen, w.inv_s, w.lp2, jd, d, w.sg, w.A,
+                                         w.lug, cfull, lml, lma, c.lattice.delay_penalty};
+                joint_stats_delay_kernel<true><<<sgrid, 256, 0, s>>>(w.part, slices, epi);
+            }
         }
     }
     // lattice: the dense path's fp32 wavefront, with the default ring depth and no PDL
@@ -1316,6 +1371,92 @@ rnntStatus_t rnnt_b200_backward_ex(int dtype, const void* activations, void* gra
                           nullptr, workspace, options}, backward_call(grad_scale, grad_costs_device, grad_options));
 }
 
+// ---- lattice options (delay penalty, DESIGN.md §10) for every storage type ---------------------------------
+rnntStatus_t rnnt_b200_loss_async_lat(int dtype, int layout, const void* activations, void* gradients,
+                                      const int* flat_labels, const int* label_lengths,
+                                      const int* input_lengths, int alphabet_size, int minibatch,
+                                      void* costs_device, double grad_scale, rnntGradOptions grad_options,
+                                      rnntLatticeOptions lattice_options, void* workspace, rnntOptions options) {
+    const bool tunv = layout == RNNT_B200_LAYOUT_TUNV;
+    if (!is_layout(layout) || (tunv && is_16bit(dtype))) return RNNT_STATUS_INVALID_VALUE;
+    Call c = full_call(grad_scale, true, tunv, grad_options);
+    c.lattice = lattice_options;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, c);
+}
+
+rnntStatus_t rnnt_b200_forward_lat(int dtype, const void* activations, const int* flat_labels,
+                                   const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                   int minibatch, void* costs_device, int prepare_backward,
+                                   rnntLatticeOptions lattice_options, void* workspace, rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.lattice = lattice_options;
+    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, c);
+}
+
+rnntStatus_t rnnt_b200_backward_lat(int dtype, const void* activations, void* gradients,
+                                    const int* flat_labels, const int* label_lengths,
+                                    const int* input_lengths, int alphabet_size, int minibatch,
+                                    const void* grad_costs_device, double grad_scale,
+                                    rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
+                                    void* workspace, rnntOptions options) {
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
+    c.lattice = lattice_options;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options}, c);
+}
+
+rnntStatus_t rnnt_b200_pruned_loss_async_lat(int dtype, int layout, const void* activations, void* gradients,
+                                             const int* ranges, int s_range, const int* flat_labels,
+                                             const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                             int minibatch, void* costs_device, double grad_scale,
+                                             rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
+                                             void* workspace, rnntOptions options) {
+    if (!is_layout(layout)) return RNNT_STATUS_INVALID_VALUE;
+    Call c = full_call(grad_scale, true, layout == RNNT_B200_LAYOUT_TUNV, grad_options);
+    c.pruned = true;
+    c.lattice = lattice_options;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options, ranges, s_range}, c);
+}
+
+rnntStatus_t rnnt_b200_pruned_forward_lat(int dtype, const void* activations, const int* ranges, int s_range,
+                                          const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                          int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
+                                          rnntLatticeOptions lattice_options, void* workspace, rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.pruned = true;
+    c.lattice = lattice_options;
+    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options, ranges, s_range}, c);
+}
+
+rnntStatus_t rnnt_b200_pruned_backward_lat(int dtype, const void* activations, void* gradients, const int* ranges,
+                                           int s_range, const int* flat_labels, const int* label_lengths,
+                                           const int* input_lengths, int alphabet_size, int minibatch,
+                                           const void* grad_costs_device, double grad_scale,
+                                           rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
+                                           void* workspace, rnntOptions options) {
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
+    c.pruned = true;
+    c.lattice = lattice_options;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options, ranges, s_range}, c);
+}
+
+// the joint's forward with smoothing and lattice options; the backward entries read the penalised factors
+rnntStatus_t rnnt_b200_add_joint_forward_lat(const float* trans, const float* pred, const int* flat_labels,
+                                             const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                             int minibatch, float* costs_device, int prepare_backward,
+                                             rnntSmoothOptions smooth, rnntLatticeOptions lattice_options,
+                                             void* workspace, rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.smooth = smooth;
+    c.lattice = lattice_options;
+    return run_add_joint({trans, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, pred, nullptr, c);
+}
 // ---- additive joint network, logits never materialised -------------------------------------------
 rnntStatus_t rnnt_b200_add_joint_loss(const float* trans, const float* pred, float* grad_trans,
                                       float* grad_pred, const int* flat_labels,

@@ -227,7 +227,9 @@ struct EpiPartial {
 // ---- J2 epilogue: S -> lse, lattice log-prob pair (diagonal-major), keep 1/S -----------------------
 // SMOOTH (DESIGN.md §9): each factor is  c lp_c + lml lp_l + lma lp_a  (a term with scale 0 is left out), with
 //   lp_c = f_k + g_k - lse,  lp_l = g_k - mg - log sg,  lp_a = f_k + log ug_k - mf - log A.
-template <bool SMOOTH = false>
+// DELAY (DESIGN.md §10): the label factor gains  delay ((T_b - 1)/2 - t)  after the smoothing interpolation, as in
+// k2; joint_stats_delay_kernel runs it.  Everything downstream reads the penalised factors from lp2.
+template <bool SMOOTH = false, bool DELAY = false>
 struct EpiStats {
     const float *f, *g, *mf, *mg;
     const int *labels, *xlen, *ylen;
@@ -237,6 +239,7 @@ struct EpiStats {
     Dims d;        // lattice geometry (maxT = T, maxU = U)
     const float *sg, *A, *lug;   // SMOOTH: [N,U] row sums of Eg, [N,T] Ef . ug, [V] log ug
     float c, lml, lma;           // SMOOTH: the three scales
+    float delay;                 // DELAY: lambda
     __device__ float mix(const float* fr, const float* gr, int k, float lse, float Lg, float La) const {
         const float fk = __ldg(fr + k), gk = __ldg(gr + k);
         float lp = 0.0f;
@@ -265,6 +268,7 @@ struct EpiStats {
             const float lpb = mix(fr, gr, jd.blank, lse, Lg, La);
             float lpl = 0.0f;
             if (has_label) lpl = mix(fr, gr, __ldg(labels + (size_t)b * (jd.U > 1 ? jd.U - 1 : 0) + u), lse, Lg, La);
+            if (DELAY && has_label) lpl += delay * delay_bracket<float>(Tb, (uint32_t)t);
             lp2[skew(d, b, t, u)] = make_fac(lpb, lpl, has_label);
             return;
         }
@@ -273,14 +277,14 @@ struct EpiStats {
         if (has_label) {
             const int y = __ldg(labels + (size_t)b * (jd.U > 1 ? jd.U - 1 : 0) + u);
             lpl = (__ldg(fr + y) + __ldg(gr + y)) - lse;
+            if (DELAY) lpl += delay * delay_bracket<float>(Tb, (uint32_t)t);
         }
         lp2[skew(d, b, t, u)] = make_fac(lpb, lpl, has_label);
     }
 };
 
-template <bool SMOOTH = false>
-__global__ void __launch_bounds__(256)
-joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats<SMOOTH> epi) {
+template <typename Epi>
+__device__ __forceinline__ void joint_stats(const float* __restrict__ part, int slices, const Epi& epi) {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= epi.d.rows) return;
     uint32_t bt, u, b, t;
@@ -289,6 +293,16 @@ joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats<SM
     float S = 0.0f;
     for (int ks = 0; ks < slices; ++ks) S += part[(size_t)ks * epi.d.rows + r];
     epi((int)b, (int)t, (int)u, S);
+}
+template <bool SMOOTH = false>
+__global__ void __launch_bounds__(256)
+joint_stats_kernel(const float* __restrict__ part, int slices, const EpiStats<SMOOTH> epi) {
+    joint_stats(part, slices, epi);
+}
+template <bool SMOOTH = false>
+__global__ void __launch_bounds__(256)
+joint_stats_delay_kernel(const float* __restrict__ part, int slices, const EpiStats<SMOOTH, true> epi) {
+    joint_stats(part, slices, epi);
 }
 
 // ---- J3: per cell weights from the lattices ---------------------------------------------------------

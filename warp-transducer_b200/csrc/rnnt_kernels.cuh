@@ -77,7 +77,7 @@ struct Prune {
 // row -> (b, t, u).  Pruned: u is ranges + s in 32-bit two's complement; a negative or too large u lands at or
 // above 2^31 as unsigned, where row_padding() catches it together with u >= U_b
 template <bool PRUNED>
-__device__ __forceinline__ void row_decode(const Dims& d, const Prune& p, uint32_t r, uint32_t& b, uint32_t& t,
+__device__ __forceinline__ void row_decode(const Dims d, const Prune p, uint32_t r, uint32_t& b, uint32_t& t,
                                            uint32_t& u) {
     if constexpr (PRUNED) {
         uint32_t bt, s;
@@ -105,6 +105,15 @@ __device__ __forceinline__ bool pruned_grad_padding(uint32_t t, uint32_t u, int 
     return row_padding<true>(t, u, Tb, Ub) || ll_dead(llf, b);
 }
 
+// ---- delay penalty (DESIGN.md §10) ----------------------------------------------------------------------
+// Each streaming kernel has a twin *_delay_kernel running the same body at DELAY = true.  Pass 1 adds
+// lambda ((T_b - 1)/2 - t) to the label log-factor of every cell with a label transition; pass 2 adds the same
+// penalty, in the exp2 domain, to the label offset cL.  The bracket is exact in T (t < 2^24), so the only
+// rounding is the product with lambda.  The plain kernels run the body at DELAY = false and keep their code.
+template <typename T> __device__ __forceinline__ T delay_bracket(int Tb, uint32_t t) {
+    return T(Tb - 1) * T(0.5) - T(t);
+}
+
 // Pruned calls start from log-zero factors everywhere, so that a cell no row covers has neither transition; pass 1
 // then writes the covered cells.  (has_label = true: the fp64 factor keeps its label log-prob only then.)
 template <typename T>
@@ -130,12 +139,12 @@ template <typename IO> struct RowThreads { static constexpr int value = sizeof(I
 #ifndef RNNT_ROWSTATS_MINB
 #define RNNT_ROWSTATS_MINB 7
 #endif
-template <typename T, int VEC, int NV, typename IO, bool PRUNED>
-__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_ROWSTATS_MINB : 8))
-rowstats_row_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
-                    const int* __restrict__ xlen, const int* __restrict__ ylen,
-                    typename Real<T>::pair* __restrict__ stat, typename Lat<T>::fac* __restrict__ lp2,
-                    const Dims d, const Prune p) {
+template <typename T, int VEC, int NV, typename IO, bool PRUNED, bool DELAY>
+__device__ __forceinline__ void rowstats_row(const IO* __restrict__ acts, const int* __restrict__ labels,
+                                             const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                             typename Real<T>::pair* __restrict__ stat,
+                                             typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p,
+                                             const T delay) {
     using R = Real<T>;
     constexpr int kRowThreads = RowThreads<IO>::value;
     __shared__ T sh_m[kRowThreads / 32], sh_s[kRowThreads / 32];
@@ -248,10 +257,27 @@ rowstats_row_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
             if (has_label) {
                 const int y = __ldg(labels + (size_t)b * (d.maxU - 1) + u);
                 lpl = (ld_scalar<T>(row + y) - M) - lse;
+                if (DELAY) lpl += delay * delay_bracket<T>(Tb, t);
             }
             lp2[skew(d, b, t, u)] = Lat<T>::make(lpb, lpl, has_label);
         }
     }
+}
+template <typename T, int VEC, int NV, typename IO, bool PRUNED>
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_ROWSTATS_MINB : 8))
+rowstats_row_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
+                    const int* __restrict__ xlen, const int* __restrict__ ylen,
+                    typename Real<T>::pair* __restrict__ stat, typename Lat<T>::fac* __restrict__ lp2,
+                    const Dims d, const Prune p) {
+    rowstats_row<T, VEC, NV, IO, PRUNED, false>(acts, labels, xlen, ylen, stat, lp2, d, p, T(0));
+}
+template <typename T, int VEC, int NV, typename IO, bool PRUNED>
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_ROWSTATS_MINB : 8))
+rowstats_row_delay_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
+                          const int* __restrict__ xlen, const int* __restrict__ ylen,
+                          typename Real<T>::pair* __restrict__ stat, typename Lat<T>::fac* __restrict__ lp2,
+                          const Dims d, const Prune p, const T delay) {
+    rowstats_row<T, VEC, NV, IO, PRUNED, true>(acts, labels, xlen, ylen, stat, lp2, d, p, delay);
 }
 
 // =================================================================================================
@@ -266,12 +292,12 @@ rowstats_row_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
 #endif
 constexpr int kVPL = RNNT_VPL;
 
-template <typename T, int VEC, int LPR, typename IO, bool PRUNED>
-__global__ void __launch_bounds__(256)
-rowstats_tile_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
-                     const int* __restrict__ xlen, const int* __restrict__ ylen,
-                     typename Real<T>::pair* __restrict__ stat,
-                     typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p) {
+template <typename T, int VEC, int LPR, typename IO, bool PRUNED, bool DELAY>
+__device__ __forceinline__ void rowstats_tile(const IO* __restrict__ acts, const int* __restrict__ labels,
+                                              const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                              typename Real<T>::pair* __restrict__ stat,
+                                              typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p,
+                                              const T delay) {
     using R = Real<T>;
     constexpr int RPW = kWarp / LPR;
     const int lane = threadIdx.x & 31;
@@ -328,10 +354,27 @@ rowstats_tile_kernel(const IO* __restrict__ acts, const int* __restrict__ labels
             if (has_label) {
                 const int y = __ldg(labels + (size_t)b * (d.maxU - 1) + u);
                 lpl = (ld_scalar<T>(row + y) - M) - lse;
+                if (DELAY) lpl += delay * delay_bracket<T>(Tb, t);
             }
             lp2[skew(d, b, t, u)] = Lat<T>::make(lpb, lpl, has_label);
         }
     }
+}
+template <typename T, int VEC, int LPR, typename IO, bool PRUNED>
+__global__ void __launch_bounds__(256)
+rowstats_tile_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
+                     const int* __restrict__ xlen, const int* __restrict__ ylen,
+                     typename Real<T>::pair* __restrict__ stat,
+                     typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p) {
+    rowstats_tile<T, VEC, LPR, IO, PRUNED, false>(acts, labels, xlen, ylen, stat, lp2, d, p, T(0));
+}
+template <typename T, int VEC, int LPR, typename IO, bool PRUNED>
+__global__ void __launch_bounds__(256)
+rowstats_tile_delay_kernel(const IO* __restrict__ acts, const int* __restrict__ labels,
+                           const int* __restrict__ xlen, const int* __restrict__ ylen,
+                           typename Real<T>::pair* __restrict__ stat,
+                           typename Lat<T>::fac* __restrict__ lp2, const Dims d, const Prune p, const T delay) {
+    rowstats_tile<T, VEC, LPR, IO, PRUNED, true>(acts, labels, xlen, ylen, stat, lp2, d, p, delay);
 }
 
 // =================================================================================================
@@ -562,6 +605,13 @@ __device__ __forceinline__ void fastemit_fold(RowGrad<T>& g, const GradReg<T>& r
     if (mx > R::neg_inf()) g.cA = mx + log2_of(R::exp2(g.cA - mx) + R::exp2(c - mx));
     g.cL += reg.log2_1p_lam;
 }
+// delay penalty of the label offset (DESIGN.md §10), after fastemit_fold: FastEmit's log2 p_y comes from the
+// stored, penalised factor, and adding it to the unpenalised cL gives exactly log2(e_y e^-lse) of the penalised
+// lattice.  delay_log2 = lambda log2(e).  A row without a label keeps cL = -inf.
+template <typename T>
+__device__ __forceinline__ void delay_fold(RowGrad<T>& g, const T delay_log2, int Tb, uint32_t t) {
+    g.cL += delay_log2 * delay_bracket<T>(Tb, t);
+}
 // clip to [-c, c]; a NaN gradient stays NaN (the c = +inf of "off" then leaves every value unchanged)
 __device__ __forceinline__ float clip_grad(float g, float c) {
     float r;
@@ -710,14 +760,15 @@ __device__ __forceinline__ RowGrad<float> row_grad_setup_spec(const Dims& d, uin
 #ifndef RNNT_GRAD_MINB16
 #define RNNT_GRAD_MINB16 8   // 16-bit rows are one trip of 128 threads: residency (bytes in flight) is what pays
 #endif
-template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED>
-__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
-grad_row_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                const int* __restrict__ xlen, const int* __restrict__ ylen,
-                const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
-                const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
-                const Prune p) {
+template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED, bool DELAY>
+__device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __restrict__ grads,
+                                         const int* __restrict__ labels, const int* __restrict__ xlen,
+                                         const int* __restrict__ ylen, const typename Real<T>::pair* __restrict__ stat,
+                                         const typename Lat<T>::val* __restrict__ alphas,
+                                         const typename Lat<T>::val* __restrict__ betas,
+                                         const typename Lat<T>::val* __restrict__ llf, const T scale_in,
+                                         const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                                         const Prune p, const T delay_log2) {
     constexpr int kRowThreads = RowThreads<IO>::value;
     const uint32_t r = d.rows - 1 - blockIdx.x;
     uint32_t u, b, t;
@@ -751,6 +802,7 @@ grad_row_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* 
     pdl_wait();         // (PDL) the logits were read ahead of the lattice kernel's completion; its output is not
     RowGrad<T> rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
     if constexpr (REG) fastemit_fold(rg, reg, b, t, u, d);
+    if constexpr (DELAY) delay_fold(rg, delay_log2, Tb, t);
     // 16-bit storage: fold the row maximum into the three offsets, one FFMA per element instead of FADD + FFMA
     // (its rounding, |m| * 6e-8 in the exponent, is far below the 16-bit quantisation of input and output)
     constexpr bool ZEROM = sizeof(IO) == 2;
@@ -774,16 +826,39 @@ grad_row_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* 
         emit(base);
     }
 }
+template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED>
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
+grad_row_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                const int* __restrict__ xlen, const int* __restrict__ ylen,
+                const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                const Prune p) {
+    grad_row<T, VEC, NV, SCALED, IO, REG, PRUNED, false>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                         scale_in, scale_vec, d, reg, p, T(0));
+}
+template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED>
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
+grad_row_delay_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                      const int* __restrict__ xlen, const int* __restrict__ ylen,
+                      const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                      const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                      const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                      const Prune p, const T delay_log2) {
+    grad_row<T, VEC, NV, SCALED, IO, REG, PRUNED, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                        scale_in, scale_vec, d, reg, p, delay_log2);
+}
 
 // Pass 2, short rows: same register tile as rowstats_tile_kernel.
-template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED>
-__global__ void __launch_bounds__(256)
-grad_tile_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
-                 const int* __restrict__ xlen, const int* __restrict__ ylen,
-                 const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
-                 const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
-                 const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
-                 const Prune p) {
+template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED, bool DELAY>
+__device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __restrict__ grads,
+                                          const int* __restrict__ labels, const int* __restrict__ xlen,
+                                          const int* __restrict__ ylen, const typename Real<T>::pair* __restrict__ stat,
+                                          const typename Lat<T>::val* __restrict__ alphas,
+                                          const typename Lat<T>::val* __restrict__ betas,
+                                          const typename Lat<T>::val* __restrict__ llf, const T scale_in,
+                                          const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                                          const Prune p, const T delay_log2) {
     constexpr int RPW = kWarp / LPR;
     const int lane = threadIdx.x & 31;
     const int sub = lane / LPR, sl = lane % LPR;
@@ -822,6 +897,7 @@ grad_tile_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int*
         pdl_wait();
         RowGrad<T> rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
         if constexpr (REG) fastemit_fold(rg, reg, b, t, u, d);
+        if constexpr (DELAY) delay_fold(rg, delay_log2, Tb, t);
 #pragma unroll
         for (int j = 0; j < kVPL; ++j) {
             const int i = sl + j * LPR;
@@ -830,6 +906,28 @@ grad_tile_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int*
                                   grad_vec<T, VEC, SCALED, false, REG>(x[j], rg, i * VEC, kb, scale, reg.clamp));
         }
     } while (false);
+}
+template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED>
+__global__ void __launch_bounds__(256)
+grad_tile_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                 const int* __restrict__ xlen, const int* __restrict__ ylen,
+                 const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                 const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                 const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                 const Prune p) {
+    grad_tile<T, VEC, LPR, SCALED, IO, REG, PRUNED, false>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                           scale_in, scale_vec, d, reg, p, T(0));
+}
+template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED>
+__global__ void __launch_bounds__(256)
+grad_tile_delay_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                       const int* __restrict__ xlen, const int* __restrict__ ylen,
+                       const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                       const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                       const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                       const Prune p, const T delay_log2) {
+    grad_tile<T, VEC, LPR, SCALED, IO, REG, PRUNED, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                          scale_in, scale_vec, d, reg, p, delay_log2);
 }
 
 }  // namespace b200rnnt

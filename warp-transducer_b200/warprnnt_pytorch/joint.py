@@ -14,6 +14,9 @@ lattice, per-logit gradients never exist to be clipped) and raises ValueError.
 The keyword-only ``lm_only_scale`` and ``am_only_scale`` give k2's smoothed loss (rnnt_loss_smoothed, the "simple"
 loss of pruned RNN-T): every lattice factor becomes  c lp_joint + lm_only_scale lp_lm + am_only_scale lp_am  with
 c = 1 - lm_only_scale - am_only_scale (include/rnnt.h, rnntSmoothOptions; DESIGN.md §9).  Both 0 is the plain loss.
+
+The keyword-only ``delay_penalty`` is RNNTLoss's: each label factor at frame t gains delay_penalty * ((T_b - 1)/2 - t),
+added after the smoothing interpolation (DESIGN.md §10); the loss includes it and the gradients are exact.
 """
 import ctypes as C
 import math
@@ -54,6 +57,9 @@ _lib.rnnt_b200_add_joint_smoothed_workspace_size.argtypes = [C.c_int, C.c_int, C
 _lib.rnnt_b200_add_joint_smoothed_forward.restype = C.c_int
 _lib.rnnt_b200_add_joint_smoothed_forward.argtypes = [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int,
                                                       rnntSmoothOptions, _P, warp_rnnt.rnntOptions]
+_lib.rnnt_b200_add_joint_forward_lat.restype = C.c_int
+_lib.rnnt_b200_add_joint_forward_lat.argtypes = [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, rnntSmoothOptions,
+                                                 warp_rnnt.rnntLatticeOptions, _P, warp_rnnt.rnntOptions]
 _lib.rnnt_b200_add_joint_smoothed_backward.restype = C.c_int
 _lib.rnnt_b200_add_joint_smoothed_backward.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_float,
                                                        warp_rnnt.rnntGradOptions, rnntSmoothOptions, _P,
@@ -129,9 +135,10 @@ def _joint_opts(trans, pred, blank):
 _lab_ptr = warp_rnnt._labels_ptr   # cached per-device stand-in when there are no labels (U == 1)
 
 
-def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare_backward, blank, smooth):
+def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare_backward, blank, smooth, lattice=None):
     """The forward half on CUDA tensors (no checks): rnnt_b200_add_joint_forward, or its smoothed form when
-    `smooth` (an rnntSmoothOptions) is given.  Returns the workspace the backward half and the ranges read."""
+    `smooth` (an rnntSmoothOptions) is given, or rnnt_b200_add_joint_forward_lat when `lattice` (an
+    rnntLatticeOptions) is given.  Returns the workspace the backward half and the ranges read."""
     N, T, V = trans.shape
     U = pred.shape[1]
     n = C.c_size_t(0)
@@ -143,7 +150,10 @@ def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare
     args = (trans.data_ptr(), pred.data_ptr(), _lab_ptr(labels), label_lens.data_ptr(), act_lens.data_ptr(), V, N,
             costs.data_ptr(), 1 if prepare_backward else 0)
     tail = (ws.data_ptr(), _joint_opts(trans, pred, blank))
-    if smooth is None:
+    if lattice is not None:
+        st = _lib.rnnt_b200_add_joint_forward_lat(*args, smooth if smooth is not None else rnntSmoothOptions(),
+                                                  lattice, *tail)
+    elif smooth is None:
         st = _lib.rnnt_b200_add_joint_forward(*args, *tail)
     else:
         st = _lib.rnnt_b200_add_joint_smoothed_forward(*args, smooth, *tail)
@@ -154,8 +164,8 @@ def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare
 
 def check_joint_call(trans, pred, labels, act_lens, label_lens, reduction, fastemit_lambda, lm_only_scale,
                      am_only_scale):
-    """Every argument rule of a joint call, before any device work: (gradient options, smoothing options,
-    deferred length check)."""
+    """Every argument rule of a joint call, before any device work but the delay penalty's (lattice_options):
+    (gradient options, smoothing options, deferred length check)."""
     gopt = warp_rnnt.grad_options(fastemit_lambda)   # ValueError before any device work
     if gopt is not None:
         gopt.clamp = 0.0                              # the joint entry accepts no clamp at all
@@ -175,7 +185,8 @@ class _AddJointRNNT(Function):
 
     @staticmethod
     def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0,
-                lm_only_scale=0.0, am_only_scale=0.0):
+                lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
+        lattice = warp_rnnt.lattice_options(delay_penalty)   # ValueError before any device work
         gopt, smooth, length_check = check_joint_call(trans, pred, labels, act_lens, label_lens, reduction,
                                                       fastemit_lambda, lm_only_scale, am_only_scale)
         N = trans.shape[0]
@@ -183,7 +194,7 @@ class _AddJointRNNT(Function):
         need = trans.requires_grad or pred.requires_grad
         costs = torch.empty(N, dtype=torch.float32, device=trans.device)
         with torch.cuda.device(trans.device):
-            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, need, blank, smooth)
+            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, need, blank, smooth, lattice)
         length_check.finish()   # the reference's length test, waited for with the kernels already queued
         if need:
             ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
@@ -215,7 +226,7 @@ class _AddJointRNNT(Function):
                 st = _lib.rnnt_b200_add_joint_backward(*args, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_add_joint_backward failed: " + warp_rnnt.status_string(st))
-        return dtrans, dpred, None, None, None, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None, None, None, None
 
 
 def _no_clamp(clamp):
@@ -225,24 +236,27 @@ def _no_clamp(clamp):
 
 
 def add_joint_rnnt_loss(trans, pred, labels, act_lens, label_lens, blank=0, reduction='mean', *,
-                        fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0, am_only_scale=0.0):
+                        fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
     """fastemit_lambda: as rnnt_loss (the gradient is then not the gradient of the returned loss).
-    lm_only_scale, am_only_scale: the smoothed loss (module docstring); both 0 is the plain loss."""
+    lm_only_scale, am_only_scale: the smoothed loss (module docstring); both 0 is the plain loss.
+    delay_penalty: as rnnt_loss, added after the smoothing (module docstring)."""
     _no_clamp(clamp)
     return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
-                               lm_only_scale, am_only_scale)
+                               lm_only_scale, am_only_scale, delay_penalty)
 
 
 class AddJointRNNTLoss(Module):
     def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0,
-                 am_only_scale=0.0):
+                 am_only_scale=0.0, delay_penalty=0.0):
         super().__init__()
         _no_clamp(clamp)
         warp_rnnt.grad_options(fastemit_lambda)
         smooth_options(lm_only_scale, am_only_scale)
+        warp_rnnt.lattice_options(delay_penalty)
         self.blank, self.reduction, self.fastemit_lambda = blank, reduction, fastemit_lambda
         self.lm_only_scale, self.am_only_scale = lm_only_scale, am_only_scale
+        self.delay_penalty = delay_penalty
 
     def forward(self, trans, pred, labels, act_lens, label_lens):
         return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, self.blank, self.reduction,
-                                   self.fastemit_lambda, self.lm_only_scale, self.am_only_scale)
+                                   self.fastemit_lambda, self.lm_only_scale, self.am_only_scale, self.delay_penalty)

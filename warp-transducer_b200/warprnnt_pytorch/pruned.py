@@ -37,6 +37,16 @@ _lib.rnnt_b200_pruned_forward.argtypes = [C.c_int, _P, _P, C.c_int, _P, _P, _P, 
 _lib.rnnt_b200_pruned_backward_ex.restype = C.c_int
 _lib.rnnt_b200_pruned_backward_ex.argtypes = [C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P,
                                               C.c_double, _GOpt, _P, _Opt]
+_LOpt = warp_rnnt.rnntLatticeOptions
+_lib.rnnt_b200_pruned_forward_lat.restype = C.c_int
+_lib.rnnt_b200_pruned_forward_lat.argtypes = [C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int,
+                                              _LOpt, _P, _Opt]
+_lib.rnnt_b200_pruned_backward_lat.restype = C.c_int
+_lib.rnnt_b200_pruned_backward_lat.argtypes = [C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P,
+                                               C.c_double, _GOpt, _LOpt, _P, _Opt]
+_lib.rnnt_b200_pruned_loss_async_lat.restype = C.c_int
+_lib.rnnt_b200_pruned_loss_async_lat.argtypes = [C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int,
+                                                 C.c_int, _P, C.c_double, _GOpt, _LOpt, _P, _Opt]
 _lib.rnnt_b200_add_joint_prune_ranges.restype = C.c_int
 _lib.rnnt_b200_add_joint_prune_ranges.argtypes = [_P, _P, C.c_int, C.c_int, _P, _P, _Opt]
 _lib.rnnt_b200_add_joint_workspace_size.restype = C.c_int
@@ -56,10 +66,11 @@ class _AddJointRNNTRanges(Function):
 
     @staticmethod
     def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, s_range,
-                lm_only_scale=0.0, am_only_scale=0.0):
+                lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
         s_range = int(s_range)
         if s_range < 2:
             raise ValueError("s_range must be >= 2, got %d" % s_range)
+        lattice = warp_rnnt.lattice_options(delay_penalty)
         gopt, smooth, length_check = check_joint_call(trans, pred, labels, act_lens, label_lens, reduction,
                                                       fastemit_lambda, lm_only_scale, am_only_scale)
         N, T = trans.shape[0], trans.shape[1]
@@ -67,7 +78,7 @@ class _AddJointRNNTRanges(Function):
         costs = torch.empty(N, dtype=torch.float32, device=trans.device)
         ranges = torch.empty((N, T), dtype=torch.int32, device=trans.device)
         with torch.cuda.device(trans.device):
-            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, True, blank, smooth)
+            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, True, blank, smooth, lattice)
             st = _lib.rnnt_b200_add_joint_prune_ranges(label_lens.data_ptr(), act_lens.data_ptr(), N, s_range,
                                                        ranges.data_ptr(), ws.data_ptr(),
                                                        _joint_opts(trans, pred, blank))
@@ -87,18 +98,19 @@ class _AddJointRNNTRanges(Function):
     @staticmethod
     def backward(ctx, grad_output, grad_ranges):
         dtrans, dpred = _AddJointRNNT.backward(ctx, grad_output)[:2]
-        return dtrans, dpred, None, None, None, None, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None, None, None, None, None
 
 
 def add_joint_rnnt_loss_with_ranges(trans, pred, labels, act_lens, label_lens, s_range, blank=0, reduction='mean',
-                                    *, fastemit_lambda=0.0, lm_only_scale=0.0, am_only_scale=0.0):
+                                    *, fastemit_lambda=0.0, lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
     """(loss, ranges): add_joint_rnnt_loss (the "simple" loss of pruned RNN-T; differentiable in trans and pred
     exactly as add_joint_rnnt_loss) and the [N, T] int32 window starts of the pruned loss for R = s_range >= 2,
     from the same forward (include/rnnt.h, rnnt_b200_add_joint_prune_ranges, defines them).  lm_only_scale and
     am_only_scale smooth the simple loss as add_joint_rnnt_loss's do (icefall's --lm-scale / --am-scale); the
-    windows then come from the smoothed lattice."""
+    windows then come from the smoothed lattice.  delay_penalty penalises it as add_joint_rnnt_loss's does (icefall's
+    --delay-penalty), and the windows come from the penalised lattice, as k2's do."""
     return _AddJointRNNTRanges.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
-                                     s_range, lm_only_scale, am_only_scale)
+                                     s_range, lm_only_scale, am_only_scale, delay_penalty)
 
 
 def prune_joint_inputs(enc, dec, ranges, s_range):
@@ -152,8 +164,9 @@ class _PrunedRNNT(Function):
 
     @staticmethod
     def forward(ctx, logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda=0.0,
-                clamp=-1.0):
+                clamp=-1.0, delay_penalty=0.0):
         warp_rnnt.grad_options(fastemit_lambda, clamp)   # ValueError before any device work
+        lattice = warp_rnnt.lattice_options(delay_penalty)
         code = warp_rnnt._dtype_code(logits)
         if reduction not in ('none', 'sum', 'mean'):
             raise ValueError("reduction must be 'none', 'sum' or 'mean'")
@@ -166,16 +179,20 @@ class _PrunedRNNT(Function):
         with torch.cuda.device(logits.device):
             ws = torch.empty(pruned_workspace_size(T, U, R, N, 8 if logits.dtype == torch.float64 else 4),
                              dtype=torch.uint8, device=logits.device)
-            st = _lib.rnnt_b200_pruned_forward(code, logits.data_ptr(), ranges.data_ptr(), R, _lab_ptr(labels),
-                                               label_lens.data_ptr(), act_lens.data_ptr(), V, N, costs.data_ptr(),
-                                               1 if need_grad else 0, ws.data_ptr(), _opts(logits, blank, U))
+            args = (code, logits.data_ptr(), ranges.data_ptr(), R, _lab_ptr(labels), label_lens.data_ptr(),
+                    act_lens.data_ptr(), V, N, costs.data_ptr(), 1 if need_grad else 0)
+            tail = (ws.data_ptr(), _opts(logits, blank, U))
+            if lattice is None:
+                st = _lib.rnnt_b200_pruned_forward(*args, *tail)
+            else:
+                st = _lib.rnnt_b200_pruned_forward_lat(*args, lattice, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_pruned_forward failed: " + warp_rnnt.status_string(st))
         length_check.finish()
         if need_grad:
             ctx.save_for_backward(logits, labels, act_lens, label_lens, ranges)
             ctx.workspace, ctx.blank, ctx.maxU = ws, blank, U
-            ctx.fastemit_lambda, ctx.clamp = fastemit_lambda, clamp
+            ctx.fastemit_lambda, ctx.clamp, ctx.lattice = fastemit_lambda, clamp, lattice
             ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -192,34 +209,40 @@ class _PrunedRNNT(Function):
         grads = torch.empty_like(logits)   # the kernel defines every element (zeros on padding)
         gopt = warp_rnnt._ex_options(ctx.fastemit_lambda, ctx.clamp)
         with torch.cuda.device(logits.device):
-            st = _lib.rnnt_b200_pruned_backward_ex(warp_rnnt._dtype_code(logits), logits.data_ptr(), grads.data_ptr(),
-                                                   ranges.data_ptr(), R, _lab_ptr(labels), label_lens.data_ptr(),
-                                                   act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale, gopt,
-                                                   ctx.workspace.data_ptr(), _opts(logits, ctx.blank, ctx.maxU))
+            args = (warp_rnnt._dtype_code(logits), logits.data_ptr(), grads.data_ptr(), ranges.data_ptr(), R,
+                    _lab_ptr(labels), label_lens.data_ptr(), act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale, gopt)
+            tail = (ctx.workspace.data_ptr(), _opts(logits, ctx.blank, ctx.maxU))
+            if ctx.lattice is None:
+                st = _lib.rnnt_b200_pruned_backward_ex(*args, *tail)
+            else:
+                st = _lib.rnnt_b200_pruned_backward_lat(*args, ctx.lattice, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_pruned_backward_ex failed: " + warp_rnnt.status_string(st))
-        return grads, None, None, None, None, None, None, None, None
+        return grads, None, None, None, None, None, None, None, None, None
 
 
 def pruned_rnnt_loss(logits, labels, act_lens, label_lens, ranges, blank=0, reduction='mean', *,
-                     fastemit_lambda=0.0, clamp=-1.0):
+                     fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
     """Pruned RNN-T loss of logits [N, T, R, V] (fp32 / fp64 / bf16 / fp16), row (b, t, s) = lattice cell
     (t, ranges[b, t] + s); ranges [N, T] int32 on the logits' device.  labels, lengths, reduction and the gradient
     options are rnnt_loss's; the lattice is [T, max(label_lens) + 1] as there.  An utterance whose windows leave no
-    path costs +inf with a zero gradient.  With R = U and ranges == 0 this is rnnt_loss exactly."""
-    return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda, clamp)
+    path costs +inf with a zero gradient.  With R = U and ranges == 0 this is rnnt_loss exactly.  delay_penalty:
+    rnnt_loss's, on the covered cells (icefall passes the same value to the simple and the pruned loss)."""
+    return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda, clamp,
+                             delay_penalty)
 
 
 class PrunedRNNTLoss(Module):
     """Module form of pruned_rnnt_loss: PrunedRNNTLoss(blank=0, reduction='mean', *, fastemit_lambda=0.0,
-    clamp=-1.0)(logits, labels, act_lens, label_lens, ranges)."""
+    clamp=-1.0, delay_penalty=0.0)(logits, labels, act_lens, label_lens, ranges)."""
 
-    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0):
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
         super().__init__()
         warp_rnnt.grad_options(fastemit_lambda, clamp)
+        warp_rnnt.lattice_options(delay_penalty)
         self.blank, self.reduction = blank, reduction
-        self.fastemit_lambda, self.clamp = fastemit_lambda, clamp
+        self.fastemit_lambda, self.clamp, self.delay_penalty = fastemit_lambda, clamp, delay_penalty
 
     def forward(self, logits, labels, act_lens, label_lens, ranges):
         return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, self.blank, self.reduction,
-                                 self.fastemit_lambda, self.clamp)
+                                 self.fastemit_lambda, self.clamp, self.delay_penalty)

@@ -29,6 +29,11 @@ class rnntGradOptions(C.Structure):
     _fields_ = [("fastemit_lambda", C.c_float), ("clamp", C.c_float)]
 
 
+class rnntLatticeOptions(C.Structure):
+    """include/rnnt.h `struct rnntLatticeOptions` (4 bytes, by value; zero = off)."""
+    _fields_ = [("delay_penalty", C.c_float)]
+
+
 RNNT_CPU, RNNT_GPU = 0, 1
 RNNT_STATUS_SUCCESS = 0
 
@@ -75,6 +80,15 @@ _lib.rnnt_b200_loss_async_ex.argtypes = [C.c_int, C.c_int, _P, _P, _P, _P, _P, C
 _lib.rnnt_b200_backward_ex.restype = C.c_int
 _lib.rnnt_b200_backward_ex.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
                                        rnntGradOptions, _P, rnntOptions]
+_lib.rnnt_b200_loss_async_lat.restype = C.c_int
+_lib.rnnt_b200_loss_async_lat.argtypes = [C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
+                                          rnntGradOptions, rnntLatticeOptions, _P, rnntOptions]
+_lib.rnnt_b200_forward_lat.restype = C.c_int
+_lib.rnnt_b200_forward_lat.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, rnntLatticeOptions,
+                                       _P, rnntOptions]
+_lib.rnnt_b200_backward_lat.restype = C.c_int
+_lib.rnnt_b200_backward_lat.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
+                                        rnntGradOptions, rnntLatticeOptions, _P, rnntOptions]
 _lib.get_workspace_size.restype = C.c_int
 _lib.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
 _lib.get_warprnnt_version.restype = C.c_int
@@ -205,6 +219,16 @@ def grad_options(fastemit_lambda=0.0, clamp=-1.0):
     return rnntGradOptions(lam, c)
 
 
+def lattice_options(delay_penalty=0.0):
+    """Checked rnntLatticeOptions for the *_lat entries, or None when the delay penalty is off (the entries without
+    lattice options then run).  delay_penalty: finite and >= 0 (float32); 0 = off.  A negative value is an error
+    here (k2 ignores it)."""
+    lam = float(delay_penalty)
+    if not (math.isfinite(lam) and 0.0 <= lam <= _FLOAT32_MAX):
+        raise ValueError("delay_penalty must be finite and >= 0 (float32), got %r" % (delay_penalty,))
+    return None if lam == 0.0 else rnntLatticeOptions(lam)
+
+
 def _dtype_code(acts):
     code = {torch.float32: RNNT_B200_FP32, torch.float64: RNNT_B200_FP64, torch.bfloat16: RNNT_B200_BF16,
             torch.float16: RNNT_B200_FP16}.get(acts.dtype)
@@ -228,8 +252,9 @@ def _workspace(acts, T, U, N, workspace):
 
 
 def _loss_async(layout, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                grad_scale, workspace, fastemit_lambda, clamp):
+                grad_scale, workspace, fastemit_lambda, clamp, delay_penalty=0.0):
     gopt = _ex_options(fastemit_lambda, clamp)
+    lopt = lattice_options(delay_penalty)
     code = _dtype_code(acts)
     if layout == RNNT_B200_LAYOUT_TUNV and code not in (RNNT_B200_FP32, RNNT_B200_FP64):
         raise TypeError("unsupported data type %s for the time-major layout" % acts.dtype)
@@ -237,34 +262,38 @@ def _loss_async(layout, T, U, N, V, acts, labels, input_lengths, label_lengths, 
         workspace = _workspace(acts, T, U, N, workspace)
         opt = _options(acts, blank_label)
         opt.maxT, opt.maxU = T, U
-        st = _lib.rnnt_b200_loss_async_ex(code, layout, acts.data_ptr(), _ptr(grads), _labels_ptr(labels),
-                                          label_lengths.data_ptr(), input_lengths.data_ptr(), V, N,
-                                          costs.data_ptr(), grad_scale, gopt, workspace.data_ptr(), opt)
+        args = (code, layout, acts.data_ptr(), _ptr(grads), _labels_ptr(labels), label_lengths.data_ptr(),
+                input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale, gopt)
+        if lopt is None:
+            st = _lib.rnnt_b200_loss_async_ex(*args, workspace.data_ptr(), opt)
+        else:
+            st = _lib.rnnt_b200_loss_async_lat(*args, lopt, workspace.data_ptr(), opt)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_loss_async_ex failed: " + status_string(st))
     return workspace
 
 
 def gpu_rnnt_async(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                   grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0):
+                   grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
     """Extension: no host synchronisation, `costs` on the device, gradients pre-multiplied by
     `grad_scale`.  Returns the workspace tensor (keep it alive until the stream has run).
     fastemit_lambda / clamp: gradient options (see grad_options); the costs do not depend on them, and
-    with FastEmit on the gradient is not the gradient of the costs."""
+    with FastEmit on the gradient is not the gradient of the costs.  delay_penalty: the lattice option (see
+    lattice_options); it changes the costs and the gradient."""
     N, T, U, V = acts.shape
     return _loss_async(RNNT_B200_LAYOUT_NTUV, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads,
-                       blank_label, grad_scale, workspace, fastemit_lambda, clamp)
+                       blank_label, grad_scale, workspace, fastemit_lambda, clamp, delay_penalty)
 
 
 def gpu_rnnt_async_tunv(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                        grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0):
+                        grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
     """Time-major extension: `acts` / `grads` are [T, U, N, V] (the layout the reference's CPU path
     indexes for batch_first == false, cpu_rnnt.h:139-144); labels [N, U-1], lengths and costs [N].
-    fp32 / fp64, no host synchronisation.  Returns the workspace tensor.  Gradient options as
+    fp32 / fp64, no host synchronisation.  Returns the workspace tensor.  Gradient and lattice options as
     gpu_rnnt_async."""
     T, U, N, V = acts.shape
     return _loss_async(RNNT_B200_LAYOUT_TUNV, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads,
-                       blank_label, grad_scale, workspace, fastemit_lambda, clamp)
+                       blank_label, grad_scale, workspace, fastemit_lambda, clamp, delay_penalty)
 
 
 def _code16(acts):
@@ -277,10 +306,12 @@ def costs_dtype(acts):
 
 
 def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_label,
-                     prepare_backward=True, workspace=None):
+                     prepare_backward=True, workspace=None, *, delay_penalty=0.0):
     """Training-step split, first half: statistics + lattices into `workspace`, costs on the
-    device, no synchronisation.  Returns the workspace tensor (hand it to gpu_rnnt_backward)."""
+    device, no synchronisation.  Returns the workspace tensor (hand it to gpu_rnnt_backward, with the same
+    delay_penalty)."""
     N, T, U, V = acts.shape
+    lopt = lattice_options(delay_penalty)
     code = _code16(acts)
     fn = {torch.float32: _lib.rnnt_b200_forward, torch.float64: _lib.rnnt_b200_forward_fp64}.get(acts.dtype)
     if code is None and fn is None:
@@ -288,27 +319,35 @@ def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_la
     with torch.cuda.device(acts.device):
         workspace = _workspace(acts, T, U, N, workspace)
         args = (acts.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(), input_lengths.data_ptr(),
-                V, N, costs.data_ptr(), 1 if prepare_backward else 0, workspace.data_ptr(),
-                _options(acts, blank_label))
-        st = _lib.rnnt_b200_forward_16(code, *args) if code else fn(*args)
+                V, N, costs.data_ptr(), 1 if prepare_backward else 0)
+        tail = (workspace.data_ptr(), _options(acts, blank_label))
+        if lopt is not None:
+            st = _lib.rnnt_b200_forward_lat(_dtype_code(acts), *args, lopt, *tail)
+        else:
+            st = _lib.rnnt_b200_forward_16(code, *args, *tail) if code else fn(*args, *tail)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_forward failed: " + status_string(st))
     return workspace
 
 
 def gpu_rnnt_backward(acts, labels, input_lengths, label_lengths, grads, grad_costs, blank_label,
-                      grad_scale, workspace, *, fastemit_lambda=0.0, clamp=-1.0):
+                      grad_scale, workspace, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
     """Second half: grads[b] = grad_scale * grad_costs[b] * d cost[b] / d acts[b] from the lattices
     gpu_rnnt_forward left in `workspace` (grad_costs: device tensor [N] or None for ones).
     With gradient options (see grad_options): grad_scale * grad_costs[b] * clip(g[b]), g[b] the FastEmit
-    gradient when fastemit_lambda > 0."""
+    gradient when fastemit_lambda > 0.  delay_penalty: the one the forward half got."""
     N, T, U, V = acts.shape
     gopt = _ex_options(fastemit_lambda, clamp)
+    lopt = lattice_options(delay_penalty)
     code = _dtype_code(acts)
     with torch.cuda.device(acts.device):
-        st = _lib.rnnt_b200_backward_ex(code, acts.data_ptr(), grads.data_ptr(), _labels_ptr(labels),
-                                        label_lengths.data_ptr(), input_lengths.data_ptr(), V, N, _ptr(grad_costs),
-                                        grad_scale, gopt, workspace.data_ptr(), _options(acts, blank_label))
+        args = (code, acts.data_ptr(), grads.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(),
+                input_lengths.data_ptr(), V, N, _ptr(grad_costs), grad_scale, gopt)
+        tail = (workspace.data_ptr(), _options(acts, blank_label))
+        if lopt is None:
+            st = _lib.rnnt_b200_backward_ex(*args, *tail)
+        else:
+            st = _lib.rnnt_b200_backward_lat(*args, lopt, *tail)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_backward_ex failed: " + status_string(st))
     return 0
