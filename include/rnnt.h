@@ -487,6 +487,88 @@ rnntStatus_t rnnt_b200_add_joint_forward_lat(const float* trans, const float* pr
                                              struct rnntLatticeOptions lattice_options, void* workspace,
                                              struct rnntOptions options);
 
+/*
+ * Lattice topology, the `rnnt_type` argument of the *_topo entries below (k2's rnnt_type; DESIGN.md §11).
+ *   RNNT_B200_RNNT_REGULAR   the transducer of every other entry: a blank moves to the next frame, a label stays on
+ *                            the frame, so a frame may emit any number of labels.
+ *   RNNT_B200_RNNT_MODIFIED  one symbol per frame (optimized_transducer's one_sym_per_frame): every frame takes
+ *                            exactly one transition, a blank (u stays) or the label y_u (u + 1), both to the next
+ *                            frame.  With T_b, U_b = label_len + 1 after the usual clamps:
+ *                              alpha(0,0) = 0, alpha(t,u) = lse(alpha(t-1,u) + lp_blank(t-1,u),
+ *                                                               alpha(t-1,u-1) + lp_label(t-1,u-1)),
+ *                              cost = -lse(alpha(T_b-1,U_b-1) + lp_blank(T_b-1,U_b-1),
+ *                                          alpha(T_b-1,U_b-2) + lp_label(T_b-1,U_b-2)).
+ *                            An utterance with U_b - 1 > T_b has no path: its cost is +inf and its gradient is zero.
+ *                            The delay penalty, FastEmit and clamp apply as for the regular topology.
+ * Any other value returns RNNT_STATUS_INVALID_VALUE before any device access.  rnnt_type = RNNT_B200_RNNT_REGULAR
+ * runs exactly the kernels of the *_lat entry of the same name and computes the same results, bitwise.  Workspace
+ * sizes do not change.  A backward half must get the rnnt_type its forward got.
+ */
+enum { RNNT_B200_RNNT_REGULAR = 0, RNNT_B200_RNNT_MODIFIED = 1 };
+
+/* rnnt_b200_loss_async_lat, _forward_lat and _backward_lat with a topology. */
+rnntStatus_t rnnt_b200_loss_async_topo(int dtype, int layout, const void* activations, void* gradients,
+                                       const int* flat_labels, const int* label_lengths,
+                                       const int* input_lengths, int alphabet_size, int minibatch,
+                                       void* costs_device, double grad_scale, struct rnntGradOptions grad_options,
+                                       struct rnntLatticeOptions lattice_options, int rnnt_type, void* workspace,
+                                       struct rnntOptions options);
+rnntStatus_t rnnt_b200_forward_topo(int dtype, const void* activations, const int* flat_labels,
+                                    const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                    int minibatch, void* costs_device, int prepare_backward,
+                                    struct rnntLatticeOptions lattice_options, int rnnt_type, void* workspace,
+                                    struct rnntOptions options);
+rnntStatus_t rnnt_b200_backward_topo(int dtype, const void* activations, void* gradients,
+                                     const int* flat_labels, const int* label_lengths,
+                                     const int* input_lengths, int alphabet_size, int minibatch,
+                                     const void* grad_costs_device, double grad_scale,
+                                     struct rnntGradOptions grad_options, struct rnntLatticeOptions lattice_options,
+                                     int rnnt_type, void* workspace, struct rnntOptions options);
+/* rnnt_b200_pruned_loss_async_lat, _forward_lat and _backward_lat with a topology.  A modified utterance whose
+ * windows leave it no path costs +inf with a zero gradient. */
+rnntStatus_t rnnt_b200_pruned_loss_async_topo(int dtype, int layout, const void* activations, void* gradients,
+                                              const int* ranges, int s_range, const int* flat_labels,
+                                              const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                              int minibatch, void* costs_device, double grad_scale,
+                                              struct rnntGradOptions grad_options,
+                                              struct rnntLatticeOptions lattice_options, int rnnt_type,
+                                              void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_forward_topo(int dtype, const void* activations, const int* ranges, int s_range,
+                                           const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                           int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
+                                           struct rnntLatticeOptions lattice_options, int rnnt_type, void* workspace,
+                                           struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_backward_topo(int dtype, const void* activations, void* gradients, const int* ranges,
+                                            int s_range, const int* flat_labels, const int* label_lengths,
+                                            const int* input_lengths, int alphabet_size, int minibatch,
+                                            const void* grad_costs_device, double grad_scale,
+                                            struct rnntGradOptions grad_options,
+                                            struct rnntLatticeOptions lattice_options, int rnnt_type,
+                                            void* workspace, struct rnntOptions options);
+
+/* The additive joint with a topology: rnnt_b200_add_joint_forward_lat plus rnnt_type; one backward half for the
+ * plain and the smoothed joint (rnntSmoothOptions both 0 = plain) with gradient options as
+ * rnnt_b200_add_joint_backward_ex; and the pruning ranges of a modified (or regular) joint workspace.  With
+ * RNNT_B200_RNNT_MODIFIED the ranges are steps 1-3 of rnnt_b200_add_joint_prune_ranges with
+ * e_y(t,u) = exp(alpha(t,u) + lp_y(t,u) + beta(t+1,u+1) - ll).  They do not guarantee a path: a window may advance
+ * R-1 labels in one frame and a modified path one, so the pruned modified loss of an utterance may be +inf with a
+ * zero gradient (DESIGN.md §11). */
+rnntStatus_t rnnt_b200_add_joint_forward_topo(const float* trans, const float* pred, const int* flat_labels,
+                                              const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                              int minibatch, float* costs_device, int prepare_backward,
+                                              struct rnntSmoothOptions smooth,
+                                              struct rnntLatticeOptions lattice_options, int rnnt_type,
+                                              void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_add_joint_backward_topo(const float* trans, const float* pred, float* grad_trans,
+                                               float* grad_pred, const int* flat_labels, const int* label_lengths,
+                                               const int* input_lengths, int alphabet_size, int minibatch,
+                                               const float* grad_costs_device, float grad_scale,
+                                               struct rnntGradOptions grad_options, struct rnntSmoothOptions smooth,
+                                               int rnnt_type, void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_add_joint_prune_ranges_topo(const int* label_lengths, const int* input_lengths, int minibatch,
+                                                   int s_range, int* ranges, const void* workspace, int rnnt_type,
+                                                   struct rnntOptions options);
+
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug
  * builds (include/detail/cpu_rnnt.h:167-170); tests/test_gpu_round2.py does the same.  Synchronises. */

@@ -16,9 +16,11 @@ SOURCES = ["rnnt_entry.cu"]
 # every source/header under csrc/ plus the public header: editing any of them marks the .so stale
 DEPS = sorted(f for f in os.listdir(SRC) if f.endswith((".cu", ".cuh", ".h"))) + \
        [os.path.join("..", "..", "include", "rnnt.h")]
+# ptxas --split-compile=0: ptxas compiles the kernels of the translation unit on as many threads as the host has CPUs
+# (each kernel's code is the same as from one thread; only the wall time changes).
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-    "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
+    "-Xcompiler", "-fPIC", "-shared", "-cudart", "static", "-Xptxas", "--split-compile=0",
 ]
 
 

@@ -263,7 +263,7 @@ template <typename T> struct ChunkRow {
     int valid;
 };
 
-template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED, bool DELAY>
+template <typename T, int TPR, int NT, bool SCALED, bool REG, bool PRUNED, bool DELAY, bool MOD = false>
 __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __restrict__ grads,
                                            const int* __restrict__ labels, const int* __restrict__ xlen,
                                            const int* __restrict__ ylen,
@@ -311,17 +311,19 @@ __device__ __forceinline__ void grad_chunk(const T* __restrict__ acts, T* __rest
             // (addresses are in bounds for any t, u of the tensor: see the workspace slack in carve(); a pruned
             // row's u is clamped into the tensor for the addresses - the row is padding whenever that changes it)
             const uint32_t ua = PRUNED ? min(u, (uint32_t)d.maxU - 1) : u;
-            rg = row_grad_setup_spec(d, r, b, t, ua, xlen, ylen, labels, stat, alphas, betas, llf, Tb, Ub);
+            rg = row_grad_setup_spec<MOD>(d, r, b, t, ua, xlen, ylen, labels, stat, alphas, betas, llf, Tb, Ub);
             if (SCALED && scale_vec) c.scale = __ldg(scale_vec + b) * scale_in;
             if constexpr (PRUNED) v = inrange && !pruned_grad_padding(t, u, Tb, Ub, llf, b);
+            else if constexpr (MOD) v = inrange && !mod_grad_padding(t, u, Tb, Ub, llf, b);
             else v = inrange && (int)t < Tb && (int)u < Ub;
         } else {
             utt_extent(d, xlen, ylen, b, Tb, Ub);
             if constexpr (PRUNED) v = inrange && !pruned_grad_padding(t, u, Tb, Ub, llf, b);
+            else if constexpr (MOD) v = inrange && !mod_grad_padding(t, u, Tb, Ub, llf, b);
             else v = inrange && (int)t < Tb && (int)u < Ub;
             rg.m = 0, rg.cA = 0, rg.cB = R::neg_inf(), rg.cL = R::neg_inf(), rg.y = -1;
             if (v) {
-                rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
+                rg = row_grad_setup<MOD>(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
                 if (SCALED && scale_vec) c.scale = __ldg(scale_vec + b) * scale_in;
             }
         }
@@ -456,6 +458,22 @@ grad_chunk_delay_kernel(const T* __restrict__ acts, T* __restrict__ grads, const
     grad_chunk<T, TPR, NT, SCALED, REG, PRUNED, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
                                                       scale_in, scale_vec, d, hmajor, wait_ns, reg, p, delay_log2,
                                                       chunk_raw, &bar_store);
+}
+// the modified topology (DESIGN.md §11); scale, gradient options and delay penalty at run time, as grad_row_mod_kernel
+template <typename T, int TPR, int NT, bool PRUNED>
+__global__ void __launch_bounds__(NT)
+grad_chunk_mod_kernel(const T* __restrict__ acts, T* __restrict__ grads, const int* __restrict__ labels,
+                      const int* __restrict__ xlen, const int* __restrict__ ylen,
+                      const typename Real<T>::pair* __restrict__ stat,
+                      const typename Lat<T>::val* __restrict__ alphas, const typename Lat<T>::val* __restrict__ betas,
+                      const typename Lat<T>::val* __restrict__ llf, const T scale_in,
+                      const T* __restrict__ scale_vec, const Dims d, const int hmajor, const uint32_t wait_ns,
+                      const GradReg<T> reg, const Prune p, const T delay_log2) {
+    extern __shared__ __align__(128) unsigned char chunk_raw[];   // declared here: see rowstats_chunk_kernel
+    __shared__ __align__(8) unsigned long long bar_store;
+    grad_chunk<T, TPR, NT, true, true, PRUNED, true, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                           scale_in, scale_vec, d, hmajor, wait_ns, reg, p, delay_log2,
+                                                           chunk_raw, &bar_store);
 }
 
 }  // namespace b200rnnt

@@ -308,6 +308,7 @@ struct Call {
     bool pruned = false;     // logits [N,maxT,R,V] over the windows Tensors::ranges (DESIGN.md §8)
     rnntSmoothOptions smooth = {0.0f, 0.0f};   // additive joint: lm-only / am-only scales (DESIGN.md §9)
     rnntLatticeOptions lattice = {0.0f};       // delay penalty of the label factors (DESIGN.md §10)
+    int rnnt_type = RNNT_B200_RNNT_REGULAR;    // lattice topology (DESIGN.md §11)
 };
 Call full_call(double scale, bool async = true, bool tunv = false, rnntGradOptions grad = {0.0f, 0.0f}) {
     return Call{kFull, async, false, tunv, scale, nullptr, grad};
@@ -336,7 +337,8 @@ struct Tensors {
 // The checks of every compute call, all before any device access; the first that fails decides the status.
 rnntStatus_t check_call(const Tensors& t, const Call& c) {
     const rnntOptions& opt = t.opt;
-    if (!grad_options_valid(c.grad) || !smooth_valid(c.smooth) || !lattice_valid(c.lattice))
+    if (!grad_options_valid(c.grad) || !smooth_valid(c.smooth) || !lattice_valid(c.lattice) ||
+        (c.rnnt_type != RNNT_B200_RNNT_REGULAR && c.rnnt_type != RNNT_B200_RNNT_MODIFIED))
         return RNNT_STATUS_INVALID_VALUE;
     if (!t.acts || !t.labels || !t.ylen || !t.xlen || (!t.costs && c.phase != kBackward) || !t.workspace ||
         t.V <= 0 || t.N <= 0 || opt.maxT <= 0 || opt.maxU <= 0 || (c.phase == kBackward && !t.grads))
@@ -394,6 +396,7 @@ struct Group {
     bool delay;          // delay penalty on: the *_delay_kernel twins, given `pen` (pass 1) and `pen_log2` (pass 2)
     T pen;               // lambda
     T pen_log2;          // lambda log2(e)
+    bool mod;            // modified topology: the *_mod_kernel gradient kernels (DESIGN.md §11)
     bool scaled() const { return scale != T(1) || scale_vec; }
 };
 
@@ -424,6 +427,10 @@ void launch_row(const Group<T, IO>& g, int pass) {
         else if (pass == 1)
             rowstats_row_kernel<T, VEC, NV, IO, PRUNED><<<grid, block, 0, g.s>>>(
                 g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, g.pr);
+        else if (g.mod)
+            launch_k(grad_row_mod_kernel<T, VEC, NV, IO, PRUNED>, grid, block, 0, g.s, g.pdl, g.acts,
+                     g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas), static_cast<Val>(g.w.betas),
+                     static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr, g.pen_log2);
         else if (DELAY)
             launch_k(grad_row_delay_kernel<T, VEC, NV, SCALED, IO, REG, PRUNED>, grid, block, 0, g.s, g.pdl, g.acts,
                      g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas), static_cast<Val>(g.w.betas),
@@ -452,6 +459,11 @@ void launch_tile(const Group<T, IO>& g, int pass) {
         else if (pass == 1)
             rowstats_tile_kernel<T, VEC, LPR, IO, PRUNED><<<grid, 256, 0, g.s>>>(
                 g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, g.pr);
+        else if (g.mod)
+            launch_k(grad_tile_mod_kernel<T, VEC, LPR, IO, PRUNED>, dim3(grid), dim3(256), 0, g.s,
+                     g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas),
+                     static_cast<Val>(g.w.betas), static_cast<Val>(g.w.llf), g.scale, g.scale_vec, g.d, g.gr, g.pr,
+                     g.pen_log2);
         else if (DELAY)
             launch_k(grad_tile_delay_kernel<T, VEC, LPR, SCALED, IO, REG, PRUNED>, dim3(grid), dim3(256), 0, g.s,
                      g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, static_cast<Val>(g.w.alphas),
@@ -587,6 +599,10 @@ bool chunk_pass(const Group<T, T>& g, int pass) {
                 else if (pass == 1)
                     prefer_smem(rowstats_chunk_kernel<T, TPR, NT, PRUNED>)<<<grid, NT, smem, g.s>>>(
                         g.acts, g.labels, g.xlen, g.ylen, stat, lp2, g.d, hmajor, wait_ns, g.pr);
+                else if (g.mod)
+                    launch_k(prefer_smem(grad_chunk_mod_kernel<T, TPR, NT, PRUNED>), dim3(grid),
+                             dim3(NT), smem, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, al, be, llf,
+                             g.scale, g.scale_vec, g.d, hmajor, wait_ns, g.gr, g.pr, g.pen_log2);
                 else if (DELAY)
                     launch_k(prefer_smem(grad_chunk_delay_kernel<T, TPR, NT, SCALED, REG, PRUNED>), dim3(grid), dim3(NT),
                              smem, g.s, g.pdl, g.acts, g.grads, g.labels, g.xlen, g.ylen, stat, al, be, llf, g.scale,
@@ -639,9 +655,10 @@ void stream_pass(const Group<T, IO>& g, int pass) {
 // fp32 lattice: linear-domain wavefront with explicit exponents, COLS label columns per lane and a factor
 // ring `depth` diagonals deep (rnnt_lattice.cuh); alpha, and beta in a second grid row when with_beta.
 // The dense path and the additive joint share it.
+// mod: the modified topology's wavefront (DESIGN.md §11).
 void launch_lattice_lin(const float4* lp2, const int* xlen, const int* ylen, LogVal* alphas, LogVal* betas,
                         LogVal* llf, LogVal* llb, float* costs, const Dims& d, bool with_beta, int depth,
-                        cudaStream_t s, bool pdl) {
+                        cudaStream_t s, bool pdl, bool mod = false) {
     const size_t ring = lattice_ring_bytes(d.maxU, depth);
     auto launch = [&](auto kernel, int static_smem) {
         if (ring + static_smem > 48 * 1024)
@@ -649,7 +666,13 @@ void launch_lattice_lin(const float4* lp2, const int* xlen, const int* ylen, Log
         launch_k(kernel, dim3(d.N, with_beta ? 2 : 1), dim3(lattice_threads(d.maxU)), ring, s, pdl, lp2, xlen, ylen,
                  alphas, betas, llf, llb, costs, d);
     };
-    if (d.maxU <= 32) launch(lattice_lin_kernel<1, false, 8>, 64);
+    if (mod) {
+        if (d.maxU <= 32) launch(lattice_lin_mod_kernel<1, false, 8>, 64);
+        else if (d.maxU <= 64) launch(lattice_lin_mod_kernel<2, false, 8>, 64);
+        else if (depth == 32) launch(lattice_lin_mod_kernel<1, true, 32>, kLinStaticSmem);
+        else if (depth == 16) launch(lattice_lin_mod_kernel<1, true, 16>, kLinStaticSmem);
+        else launch(lattice_lin_mod_kernel<1, true, 8>, kLinStaticSmem);
+    } else if (d.maxU <= 32) launch(lattice_lin_kernel<1, false, 8>, 64);
     else if (d.maxU <= 64) launch(lattice_lin_kernel<2, false, 8>, 64);
     else if (depth == 32) launch(lattice_lin_kernel<1, true, 32>, kLinStaticSmem);
     else if (depth == 16) launch(lattice_lin_kernel<1, true, 16>, kLinStaticSmem);
@@ -765,6 +788,7 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
         g.delay = delay_on(c.lattice);
         g.pen = (T)c.lattice.delay_penalty;
         g.pen_log2 = (T)((double)c.lattice.delay_penalty * 1.4426950408889634);
+        g.mod = c.rnnt_type == RNNT_B200_RNNT_MODIFIED;
         return g;
     };
     const bool with_beta = grads || c.want_beta;
@@ -774,7 +798,7 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
             launch_lattice_lin(static_cast<const float4*>(g.w.lp2), g.xlen, g.ylen, static_cast<LogVal*>(g.w.alphas),
                                static_cast<LogVal*>(g.w.betas), static_cast<LogVal*>(g.w.llf),
                                static_cast<LogVal*>(g.w.llb), g.costs, g.d, with_beta,
-                               lattice_ring_depth(opt.maxU, co_running, hooks().lat_ring), st, g.pdl);
+                               lattice_ring_depth(opt.maxU, co_running, hooks().lat_ring), st, g.pdl, g.mod);
         } else {
             // fp64: log-domain wavefront (rnnt_kernels.cuh)
             const int threads = (opt.maxU + 31) / 32 * 32;
@@ -789,7 +813,9 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
                          static_cast<double*>(g.w.betas), static_cast<double*>(g.w.llf),
                          static_cast<double*>(g.w.llb), g.costs, g.d);
             };
-            if (threads > 32) launch(lattice_kernel<double, true>);
+            if (g.mod && threads > 32) launch(lattice_mod_kernel<double, true>);
+            else if (g.mod) launch(lattice_mod_kernel<double, false>);
+            else if (threads > 32) launch(lattice_kernel<double, true>);
             else launch(lattice_kernel<double, false>);
         }
         ++g_last_launches;
@@ -1078,7 +1104,8 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
         }
     }
     // lattice: the dense path's fp32 wavefront, with the default ring depth and no PDL
-    launch_lattice_lin(w.lp2, xlen, ylen, w.alphas, w.betas, w.llf, w.llb, costs, d, with_beta, 8, s, false);
+    launch_lattice_lin(w.lp2, xlen, ylen, w.alphas, w.betas, w.llf, w.llb, costs, d, with_beta, 8, s, false,
+                       c.rnnt_type == RNNT_B200_RNNT_MODIFIED);
     g_last_launches += 5;
     }  // phase != kBackward
     if (want_grad) {
@@ -1089,6 +1116,10 @@ rnntStatus_t run_add_joint(const Tensors& t, const float* g, float* dG, const Ca
         const unsigned wm_entries = (unsigned)N * T * wm_pitch;
         auto weights = fastemit_lambda > 0.0f ? (sm ? joint_weights_kernel<true, true> : joint_weights_kernel<true>)
                                               : (sm ? joint_weights_kernel<false, true> : joint_weights_kernel<false>);
+        if (c.rnnt_type == RNNT_B200_RNNT_MODIFIED)   // the modified topology (DESIGN.md §11)
+            weights = fastemit_lambda > 0.0f
+                          ? (sm ? joint_weights_mod_kernel<true, true> : joint_weights_mod_kernel<true>)
+                          : (sm ? joint_weights_mod_kernel<false, true> : joint_weights_mod_kernel<false>);
         weights<<<(wm_entries + 255) / 256, 256, 0, s>>>(w.lp2, w.alphas, w.betas, w.llf, w.inv_s, xlen, ylen, w.wm, w.bk,
                                                          w.lb, scale, scale_vec, d, wm_pitch, fastemit_lambda, cfull);
         // smoothing: the per-row epilogue coefficients of dF and dG, and h (the gradient through ug) when lma > 0
@@ -1371,91 +1402,181 @@ rnntStatus_t rnnt_b200_backward_ex(int dtype, const void* activations, void* gra
                           nullptr, workspace, options}, backward_call(grad_scale, grad_costs_device, grad_options));
 }
 
-// ---- lattice options (delay penalty, DESIGN.md §10) for every storage type ---------------------------------
+// ---- lattice options (delay penalty, DESIGN.md §10) and topology (DESIGN.md §11) for every storage type -----
+// The *_lat entries are the *_topo ones with the regular topology.
+rnntStatus_t rnnt_b200_loss_async_topo(int dtype, int layout, const void* activations, void* gradients,
+                                       const int* flat_labels, const int* label_lengths,
+                                       const int* input_lengths, int alphabet_size, int minibatch,
+                                       void* costs_device, double grad_scale, rnntGradOptions grad_options,
+                                       rnntLatticeOptions lattice_options, int rnnt_type, void* workspace,
+                                       rnntOptions options) {
+    const bool tunv = layout == RNNT_B200_LAYOUT_TUNV;
+    if (!is_layout(layout) || (tunv && is_16bit(dtype))) return RNNT_STATUS_INVALID_VALUE;
+    Call c = full_call(grad_scale, true, tunv, grad_options);
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, c);
+}
 rnntStatus_t rnnt_b200_loss_async_lat(int dtype, int layout, const void* activations, void* gradients,
                                       const int* flat_labels, const int* label_lengths,
                                       const int* input_lengths, int alphabet_size, int minibatch,
                                       void* costs_device, double grad_scale, rnntGradOptions grad_options,
                                       rnntLatticeOptions lattice_options, void* workspace, rnntOptions options) {
-    const bool tunv = layout == RNNT_B200_LAYOUT_TUNV;
-    if (!is_layout(layout) || (tunv && is_16bit(dtype))) return RNNT_STATUS_INVALID_VALUE;
-    Call c = full_call(grad_scale, true, tunv, grad_options);
-    c.lattice = lattice_options;
-    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          costs_device, workspace, options}, c);
+    return rnnt_b200_loss_async_topo(dtype, layout, activations, gradients, flat_labels, label_lengths, input_lengths,
+                                     alphabet_size, minibatch, costs_device, grad_scale, grad_options, lattice_options,
+                                     RNNT_B200_RNNT_REGULAR, workspace, options);
 }
 
+rnntStatus_t rnnt_b200_forward_topo(int dtype, const void* activations, const int* flat_labels,
+                                    const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                    int minibatch, void* costs_device, int prepare_backward,
+                                    rnntLatticeOptions lattice_options, int rnnt_type, void* workspace,
+                                    rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, c);
+}
 rnntStatus_t rnnt_b200_forward_lat(int dtype, const void* activations, const int* flat_labels,
                                    const int* label_lengths, const int* input_lengths, int alphabet_size,
                                    int minibatch, void* costs_device, int prepare_backward,
                                    rnntLatticeOptions lattice_options, void* workspace, rnntOptions options) {
-    Call c = forward_call(prepare_backward);
-    c.lattice = lattice_options;
-    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          costs_device, workspace, options}, c);
+    return rnnt_b200_forward_topo(dtype, activations, flat_labels, label_lengths, input_lengths, alphabet_size,
+                                  minibatch, costs_device, prepare_backward, lattice_options, RNNT_B200_RNNT_REGULAR,
+                                  workspace, options);
 }
 
+rnntStatus_t rnnt_b200_backward_topo(int dtype, const void* activations, void* gradients,
+                                     const int* flat_labels, const int* label_lengths,
+                                     const int* input_lengths, int alphabet_size, int minibatch,
+                                     const void* grad_costs_device, double grad_scale,
+                                     rnntGradOptions grad_options, rnntLatticeOptions lattice_options, int rnnt_type,
+                                     void* workspace, rnntOptions options) {
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options}, c);
+}
 rnntStatus_t rnnt_b200_backward_lat(int dtype, const void* activations, void* gradients,
                                     const int* flat_labels, const int* label_lengths,
                                     const int* input_lengths, int alphabet_size, int minibatch,
                                     const void* grad_costs_device, double grad_scale,
                                     rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
                                     void* workspace, rnntOptions options) {
-    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
-    c.lattice = lattice_options;
-    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          nullptr, workspace, options}, c);
+    return rnnt_b200_backward_topo(dtype, activations, gradients, flat_labels, label_lengths, input_lengths,
+                                   alphabet_size, minibatch, grad_costs_device, grad_scale, grad_options,
+                                   lattice_options, RNNT_B200_RNNT_REGULAR, workspace, options);
 }
 
+rnntStatus_t rnnt_b200_pruned_loss_async_topo(int dtype, int layout, const void* activations, void* gradients,
+                                              const int* ranges, int s_range, const int* flat_labels,
+                                              const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                              int minibatch, void* costs_device, double grad_scale,
+                                              rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
+                                              int rnnt_type, void* workspace, rnntOptions options) {
+    if (!is_layout(layout)) return RNNT_STATUS_INVALID_VALUE;
+    Call c = full_call(grad_scale, true, layout == RNNT_B200_LAYOUT_TUNV, grad_options);
+    c.pruned = true;
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options, ranges, s_range}, c);
+}
 rnntStatus_t rnnt_b200_pruned_loss_async_lat(int dtype, int layout, const void* activations, void* gradients,
                                              const int* ranges, int s_range, const int* flat_labels,
                                              const int* label_lengths, const int* input_lengths, int alphabet_size,
                                              int minibatch, void* costs_device, double grad_scale,
                                              rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
                                              void* workspace, rnntOptions options) {
-    if (!is_layout(layout)) return RNNT_STATUS_INVALID_VALUE;
-    Call c = full_call(grad_scale, true, layout == RNNT_B200_LAYOUT_TUNV, grad_options);
-    c.pruned = true;
-    c.lattice = lattice_options;
-    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          costs_device, workspace, options, ranges, s_range}, c);
+    return rnnt_b200_pruned_loss_async_topo(dtype, layout, activations, gradients, ranges, s_range, flat_labels,
+                                            label_lengths, input_lengths, alphabet_size, minibatch, costs_device,
+                                            grad_scale, grad_options, lattice_options, RNNT_B200_RNNT_REGULAR,
+                                            workspace, options);
 }
 
+rnntStatus_t rnnt_b200_pruned_forward_topo(int dtype, const void* activations, const int* ranges, int s_range,
+                                           const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                           int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
+                                           rnntLatticeOptions lattice_options, int rnnt_type, void* workspace,
+                                           rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.pruned = true;
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options, ranges, s_range}, c);
+}
 rnntStatus_t rnnt_b200_pruned_forward_lat(int dtype, const void* activations, const int* ranges, int s_range,
                                           const int* flat_labels, const int* label_lengths, const int* input_lengths,
                                           int alphabet_size, int minibatch, void* costs_device, int prepare_backward,
                                           rnntLatticeOptions lattice_options, void* workspace, rnntOptions options) {
-    Call c = forward_call(prepare_backward);
-    c.pruned = true;
-    c.lattice = lattice_options;
-    return run_as(dtype, {activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          costs_device, workspace, options, ranges, s_range}, c);
+    return rnnt_b200_pruned_forward_topo(dtype, activations, ranges, s_range, flat_labels, label_lengths,
+                                         input_lengths, alphabet_size, minibatch, costs_device, prepare_backward,
+                                         lattice_options, RNNT_B200_RNNT_REGULAR, workspace, options);
 }
 
+rnntStatus_t rnnt_b200_pruned_backward_topo(int dtype, const void* activations, void* gradients, const int* ranges,
+                                            int s_range, const int* flat_labels, const int* label_lengths,
+                                            const int* input_lengths, int alphabet_size, int minibatch,
+                                            const void* grad_costs_device, double grad_scale,
+                                            rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
+                                            int rnnt_type, void* workspace, rnntOptions options) {
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
+    c.pruned = true;
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options, ranges, s_range}, c);
+}
 rnntStatus_t rnnt_b200_pruned_backward_lat(int dtype, const void* activations, void* gradients, const int* ranges,
                                            int s_range, const int* flat_labels, const int* label_lengths,
                                            const int* input_lengths, int alphabet_size, int minibatch,
                                            const void* grad_costs_device, double grad_scale,
                                            rnntGradOptions grad_options, rnntLatticeOptions lattice_options,
                                            void* workspace, rnntOptions options) {
-    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
-    c.pruned = true;
-    c.lattice = lattice_options;
-    return run_as(dtype, {activations, gradients, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          nullptr, workspace, options, ranges, s_range}, c);
+    return rnnt_b200_pruned_backward_topo(dtype, activations, gradients, ranges, s_range, flat_labels, label_lengths,
+                                          input_lengths, alphabet_size, minibatch, grad_costs_device, grad_scale,
+                                          grad_options, lattice_options, RNNT_B200_RNNT_REGULAR, workspace, options);
 }
 
 // the joint's forward with smoothing and lattice options; the backward entries read the penalised factors
+rnntStatus_t rnnt_b200_add_joint_forward_topo(const float* trans, const float* pred, const int* flat_labels,
+                                              const int* label_lengths, const int* input_lengths, int alphabet_size,
+                                              int minibatch, float* costs_device, int prepare_backward,
+                                              rnntSmoothOptions smooth, rnntLatticeOptions lattice_options,
+                                              int rnnt_type, void* workspace, rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.smooth = smooth;
+    c.lattice = lattice_options;
+    c.rnnt_type = rnnt_type;
+    return run_add_joint({trans, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          costs_device, workspace, options}, pred, nullptr, c);
+}
 rnntStatus_t rnnt_b200_add_joint_forward_lat(const float* trans, const float* pred, const int* flat_labels,
                                              const int* label_lengths, const int* input_lengths, int alphabet_size,
                                              int minibatch, float* costs_device, int prepare_backward,
                                              rnntSmoothOptions smooth, rnntLatticeOptions lattice_options,
                                              void* workspace, rnntOptions options) {
-    Call c = forward_call(prepare_backward);
+    return rnnt_b200_add_joint_forward_topo(trans, pred, flat_labels, label_lengths, input_lengths, alphabet_size,
+                                            minibatch, costs_device, prepare_backward, smooth, lattice_options,
+                                            RNNT_B200_RNNT_REGULAR, workspace, options);
+}
+// the joint's backward half of any topology, with gradient and smoothing options (the forward's)
+rnntStatus_t rnnt_b200_add_joint_backward_topo(const float* trans, const float* pred, float* grad_trans,
+                                               float* grad_pred, const int* flat_labels, const int* label_lengths,
+                                               const int* input_lengths, int alphabet_size, int minibatch,
+                                               const float* grad_costs_device, float grad_scale,
+                                               rnntGradOptions grad_options, rnntSmoothOptions smooth, int rnnt_type,
+                                               void* workspace, rnntOptions options) {
+    if (grad_options.clamp != 0.0f) return RNNT_STATUS_INVALID_VALUE;   // as rnnt_b200_add_joint_backward_ex
+    Call c = backward_call(grad_scale, grad_costs_device, grad_options);
     c.smooth = smooth;
-    c.lattice = lattice_options;
-    return run_add_joint({trans, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
-                          costs_device, workspace, options}, pred, nullptr, c);
+    c.rnnt_type = rnnt_type;
+    return run_add_joint({trans, grad_trans, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+                          nullptr, workspace, options}, pred, grad_pred, c);
 }
 // ---- additive joint network, logits never materialised -------------------------------------------
 rnntStatus_t rnnt_b200_add_joint_loss(const float* trans, const float* pred, float* grad_trans,
@@ -1583,8 +1704,11 @@ rnntStatus_t rnnt_b200_pruned_backward_ex(int dtype, const void* activations, vo
                           nullptr, workspace, options, ranges, s_range}, c);
 }
 
-rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const int* input_lengths, int minibatch,
-                                              int s_range, int* ranges, const void* workspace, rnntOptions options) {
+rnntStatus_t rnnt_b200_add_joint_prune_ranges_topo(const int* label_lengths, const int* input_lengths, int minibatch,
+                                                   int s_range, int* ranges, const void* workspace, int rnnt_type,
+                                                   rnntOptions options) {
+    if (rnnt_type != RNNT_B200_RNNT_REGULAR && rnnt_type != RNNT_B200_RNNT_MODIFIED) return RNNT_STATUS_INVALID_VALUE;
+    const bool mod = rnnt_type == RNNT_B200_RNNT_MODIFIED;
     const int T = options.maxT, U = options.maxU, N = minibatch;
     if (!label_lengths || !input_lengths || !ranges || !workspace || N <= 0 || T <= 0 || U <= 0 || s_range < 2)
         return RNNT_STATUS_INVALID_VALUE;
@@ -1595,15 +1719,20 @@ rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const in
     if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
         smem > (size_t)optin)
         return RNNT_STATUS_INVALID_VALUE;   // maxT beyond ~50k frames: the window starts no longer fit on chip
+    const auto kernel = mod ? joint_prune_ranges_mod_kernel : joint_prune_ranges_kernel;
     if (smem > 48 * 1024)
-        func_attr_once(reinterpret_cast<const void*>(joint_prune_ranges_kernel),
-                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const JointWorkspace w = carve_joint(const_cast<void*>(workspace), N, T, U, 1);   // lattice sections: V-free
     Tensors t{nullptr, nullptr, nullptr, label_lengths, input_lengths, 1, N, nullptr, nullptr, options};
-    joint_prune_ranges_kernel<<<N, kRangeWarps * 32, smem, reinterpret_cast<cudaStream_t>(options.stream)>>>(
+    kernel<<<N, kRangeWarps * 32, smem, reinterpret_cast<cudaStream_t>(options.stream)>>>(
         w.lp2, w.alphas, w.betas, w.llf, input_lengths, label_lengths, ranges, make_dims(t, false), s_range);
     g_last_launches = 1;
     return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED;
+}
+rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const int* input_lengths, int minibatch,
+                                              int s_range, int* ranges, const void* workspace, rnntOptions options) {
+    return rnnt_b200_add_joint_prune_ranges_topo(label_lengths, input_lengths, minibatch, s_range, ranges, workspace,
+                                                 RNNT_B200_RNNT_REGULAR, options);
 }
 
 rnntStatus_t get_workspace_size(int maxT, int maxU, int minibatch, bool gpu, size_t* size_bytes,

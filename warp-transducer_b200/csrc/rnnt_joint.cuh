@@ -309,14 +309,16 @@ joint_stats_delay_kernel(const float* __restrict__ part, int slices, const EpiSt
 //   Wm = e^{alpha+beta-ll} / S ;  Bk = blank-transition occupancy ;  Lb = label-transition occupancy
 // REG (FastEmit, rnnt_kernels.cuh GradReg): Wm += lambda Lb / S and Lb *= 1 + lambda.
 // SMOOTH (DESIGN.md §9): Wm carries the scale c of the full-joint term; Bk / Lb stay the factor gradients.
-template <bool REG = false, bool SMOOTH = false>
-__global__ void __launch_bounds__(256)
-joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
-                     const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
-                     const float* __restrict__ inv_s, const int* __restrict__ xlen,
-                     const int* __restrict__ ylen, float* __restrict__ Wm, float* __restrict__ Bk,
-                     float* __restrict__ Lb, const float scale_in, const float* __restrict__ scale_vec,
-                     const Dims d, const int wm_pitch, const float lam, const float c) {
+// MOD (the modified topology, DESIGN.md §11): Lb reads beta(t+1,u+1) (on the last frame only u = U-2 has a label
+// transition, into the virtual beta(T,U-1) = log 1), and an utterance without a path gets zero weights.
+template <bool REG, bool SMOOTH, bool MOD>
+__device__ __forceinline__ void joint_weights(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                                              const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                                              const float* __restrict__ inv_s, const int* __restrict__ xlen,
+                                              const int* __restrict__ ylen, float* __restrict__ Wm,
+                                              float* __restrict__ Bk, float* __restrict__ Lb, const float scale_in,
+                                              const float* __restrict__ scale_vec, const Dims& d, const int wm_pitch,
+                                              const float lam, const float c) {
     // Wm rows have `wm_pitch` >= maxU entries (zero beyond maxU: the tensor-core kernel fetches them as aligned
     // float4 rows); Bk / Lb / inv_s are [N,T,maxU].  One thread per Wm entry.
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -333,7 +335,7 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
     utt_extent(d, xlen, ylen, b, Tb, Ub);
     float w = 0.0f, bk = 0.0f, lb = 0.0f;
     const float scale = scale_vec ? scale_in * __ldg(scale_vec + b) : scale_in;
-    if ((int)t < Tb && (int)u < Ub) {
+    if ((int)t < Tb && (int)u < Ub && !(MOD && ll_dead(llf, b))) {
         // everything in the exp2 domain: log2 occupancy = exact integer part + small float part
         const float4 fc = lp2[skew(d, b, t, u)];
         const size_t q = cell(d, b, t, u);
@@ -348,8 +350,10 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
         } else if ((int)u == Ub - 1) {
             bk = scale * exp2f((float)oe + ol + lpb2);
         }
-        if ((int)u < Ub - 1) {
-            const LogVal bn = betas[q + 1];
+        if ((int)u < Ub - 1 && (!MOD || (int)t < Tb - 1 || (int)u == Ub - 2)) {
+            // MOD on the last frame: the virtual beta(T,U-1), log 0 = 0, is LogVal {0, 0}
+            const bool term = MOD && (int)t == Tb - 1;
+            const LogVal bn = term ? LogVal{0, 0.0f} : betas[q + (MOD ? d.maxU + 1 : 1)];
             const float lpl2 = (float)__float_as_int(fc.w) + log2f(fc.z);
             lb = scale * exp2f((float)(oe + bn.e) + (ol + bn.l) + lpl2);
             if (REG) {
@@ -363,6 +367,28 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
     Bk[r] = bk;
     Lb[r] = lb;
 }
+template <bool REG = false, bool SMOOTH = false>
+__global__ void __launch_bounds__(256)
+joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                     const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                     const float* __restrict__ inv_s, const int* __restrict__ xlen,
+                     const int* __restrict__ ylen, float* __restrict__ Wm, float* __restrict__ Bk,
+                     float* __restrict__ Lb, const float scale_in, const float* __restrict__ scale_vec,
+                     const Dims d, const int wm_pitch, const float lam, const float c) {
+    joint_weights<REG, SMOOTH, false>(lp2, alphas, betas, llf, inv_s, xlen, ylen, Wm, Bk, Lb, scale_in, scale_vec, d,
+                                      wm_pitch, lam, c);
+}
+template <bool REG = false, bool SMOOTH = false>
+__global__ void __launch_bounds__(256)
+joint_weights_mod_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                         const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                         const float* __restrict__ inv_s, const int* __restrict__ xlen,
+                         const int* __restrict__ ylen, float* __restrict__ Wm, float* __restrict__ Bk,
+                         float* __restrict__ Lb, const float scale_in, const float* __restrict__ scale_vec,
+                         const Dims d, const int wm_pitch, const float lam, const float c) {
+    joint_weights<REG, SMOOTH, true>(lp2, alphas, betas, llf, inv_s, xlen, ylen, Wm, Bk, Lb, scale_in, scale_vec, d,
+                                     wm_pitch, lam, c);
+}
 
 // ---- pruning ranges (DESIGN.md §8) from the lattice a forward with beta left in the workspace ---------------
 // With E = max(U_b - R, 0) and the occupancies  e_b(t,u) = exp(alpha(t,u) + lp_blank(t,u) + beta(t+1,u) - ll),
@@ -374,16 +400,19 @@ joint_weights_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ 
 // One CTA per utterance.  A warp takes a frame at a time: the frame's occupancies go to the warp's shared-memory
 // rows, lane l scores the starts a = l, l+32, ... (strict > keeps its smallest best) and a shuffle argmax keeps the
 // smallest a on ties.  Thread 0 then runs the sweep over the frame starts in shared memory.
+// MOD (DESIGN.md §11): e_y(t,u) = exp(alpha(t,u) + lp_y(t,u) + beta(t+1,u+1) - ll); an utterance without a path
+// scores every start 0 (so step 1 picks a = 0).
 constexpr int kRangeWarps = 4;
 inline size_t prune_ranges_smem(int maxT, int maxU) {
     return (size_t)kRangeWarps * 2 * maxU * sizeof(float) + (size_t)maxT * sizeof(int);
 }
-__global__ void __launch_bounds__(kRangeWarps * 32)
-joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
-                          const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
-                          const int* __restrict__ xlen, const int* __restrict__ ylen, int* __restrict__ ranges,
-                          const Dims d, const int R) {
-    extern __shared__ float range_smem[];   // [kRangeWarps][2][maxU] occupancies, then [maxT] window starts
+template <bool MOD>
+__device__ __forceinline__ void joint_prune_ranges(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                                                   const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                                                   const int* __restrict__ xlen, const int* __restrict__ ylen,
+                                                   int* __restrict__ ranges, const Dims& d, const int R,
+                                                   float* range_smem) {
+    // range_smem: [kRangeWarps][2][maxU] occupancies, then [maxT] window starts
     const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int Tb, Ub;
     utt_extent(d, xlen, ylen, b, Tb, Ub);
@@ -392,8 +421,13 @@ joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restri
     float* ey = eb + d.maxU;
     int* s = reinterpret_cast<int*>(range_smem + (size_t)kRangeWarps * 2 * d.maxU);
     const LogVal ll = llf[b];
+    const bool dead = MOD && ll_dead(llf, b);
     for (int t = 1 + warp; t < Tb - 1; t += kRangeWarps) {
         for (int u = lane; u < Ub; u += 32) {
+            if (dead) {
+                eb[u] = ey[u] = 0.0f;
+                continue;
+            }
             // exp2 domain, as joint_weights_kernel: exact integer exponent + small float part
             const float4 fc = lp2[skew(d, b, t, u)];
             const size_t q = cell(d, b, t, u);
@@ -402,7 +436,7 @@ joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restri
             const float ol = a.l - ll.l;
             eb[u] = exp2f((float)(oe + bn.e) + (ol + bn.l) + ((float)__float_as_int(fc.y) + log2f(fc.x)));
             if (u < Ub - 1) {
-                const LogVal bl = betas[q + 1];
+                const LogVal bl = betas[q + (MOD ? d.maxU + 1 : 1)];
                 ey[u] = exp2f((float)(oe + bl.e) + (ol + bl.l) + ((float)__float_as_int(fc.w) + log2f(fc.z)));
             }
         }
@@ -433,6 +467,22 @@ joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restri
     }
     __syncthreads();
     for (int t = threadIdx.x; t < d.maxT; t += blockDim.x) ranges[(size_t)b * d.maxT + t] = t < Tb ? s[t] : E;
+}
+__global__ void __launch_bounds__(kRangeWarps * 32)
+joint_prune_ranges_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                          const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                          const int* __restrict__ xlen, const int* __restrict__ ylen, int* __restrict__ ranges,
+                          const Dims d, const int R) {
+    extern __shared__ float range_smem[];
+    joint_prune_ranges<false>(lp2, alphas, betas, llf, xlen, ylen, ranges, d, R, range_smem);
+}
+__global__ void __launch_bounds__(kRangeWarps * 32)
+joint_prune_ranges_mod_kernel(const float4* __restrict__ lp2, const LogVal* __restrict__ alphas,
+                              const LogVal* __restrict__ betas, const LogVal* __restrict__ llf,
+                              const int* __restrict__ xlen, const int* __restrict__ ylen, int* __restrict__ ranges,
+                              const Dims d, const int R) {
+    extern __shared__ float range_smem[];
+    joint_prune_ranges<true>(lp2, alphas, betas, llf, xlen, ylen, ranges, d, R, range_smem);
 }
 
 // ---- J4/J5: out[b,r,v] = Eout[b,r,v] * sum_s W(r,s) * Ein[b,s,v]  (thin contraction over s) ----------

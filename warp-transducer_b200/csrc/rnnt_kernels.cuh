@@ -104,6 +104,12 @@ template <typename Val>
 __device__ __forceinline__ bool pruned_grad_padding(uint32_t t, uint32_t u, int Tb, int Ub, const Val* llf, uint32_t b) {
     return row_padding<true>(t, u, Tb, Ub) || ll_dead(llf, b);
 }
+// padding of pass 2 in the dense MOD instantiations: a modified lattice (DESIGN.md §11) has no path when
+// U_b - 1 > T_b, so they ask ll_dead as the pruned ones do.  (The regular ones keep the test spelled out.)
+template <typename Val>
+__device__ __forceinline__ bool mod_grad_padding(uint32_t t, uint32_t u, int Tb, int Ub, const Val* llf, uint32_t b) {
+    return (int)t >= Tb || (int)u >= Ub || ll_dead(llf, b);
+}
 
 // ---- delay penalty (DESIGN.md §10) ----------------------------------------------------------------------
 // Each streaming kernel has a twin *_delay_kernel running the same body at DELAY = true.  Pass 1 adds
@@ -428,17 +434,19 @@ template <typename T> __device__ __forceinline__ double lse2(double x, double y)
     }
 }
 
-template <typename T, bool MULTI>
-__global__ void __launch_bounds__(1024)
-lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __restrict__ xlen,
-               const int* __restrict__ ylen, double* __restrict__ alphas,
-               double* __restrict__ betas, double* __restrict__ llf, double* __restrict__ llb,
-               T* __restrict__ costs, const Dims d) {
+// MOD: the modified topology (DESIGN.md §11).  The label term of cell (t,u) comes from (t-1,u-1) (alpha) /
+// (t+1,u+1) (beta), which the neighbouring thread held one step before the value it offers today: alpha offers
+// `off` = alpha + lp_label of its cell on the previous diagonal, beta offers `bprev` = its value of one step
+// earlier.  Alpha runs one diagonal further, to the virtual cell (T, U-1), the log-likelihood.
+template <typename T, bool MULTI, bool MOD>
+__device__ __forceinline__ void lattice_body(const typename Real<T>::pair* __restrict__ lp2, const int* __restrict__ xlen,
+                                             const int* __restrict__ ylen, double* __restrict__ alphas,
+                                             double* __restrict__ betas, double* __restrict__ llf,
+                                             double* __restrict__ llb, T* __restrict__ costs, const Dims& d,
+                                             unsigned char* ring_raw, double (*edge)[32]) {
     using P = typename Real<T>::pair;
     constexpr double NINF = -(double)INFINITY;
-    extern __shared__ __align__(16) unsigned char ring_raw[];
     P* ring = reinterpret_cast<P*>(ring_raw);  // [kRing][blockDim.x]
-    __shared__ double edge[2][32];
     const int b = blockIdx.x;
     const int u = threadIdx.x;
     const int NT = blockDim.x;
@@ -474,10 +482,11 @@ lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __rest
             fslot += NT;
         }
         unsigned rslot = u;  // slot of diagonal n-1
-        for (int n = 1; n <= last; ++n) {
+        double off = NINF, ll_mod = NINF;   // MOD only
+        for (int n = 1; n <= last + (MOD ? 1 : 0); ++n) {
             cp_async_wait<kRing - 2>();  // diagonal n-1 has landed (this thread's part)
             if (MULTI) {
-                if (lane == 31) edge[n & 1][warp] = a;
+                if (lane == 31) edge[n & 1][warp] = MOD ? off : a;
                 __syncthreads();
             } else {
                 __syncwarp();
@@ -489,10 +498,24 @@ lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __rest
             ++fdg;
             fslot += NT;
             if (fslot >= ring_elems) fslot -= ring_elems;
-            double a_left = __shfl_up_sync(0xffffffffu, a, 1);
+            double a_left = __shfl_up_sync(0xffffffffu, MOD ? off : a, 1);
             if (MULTI && lane == 0 && warp > 0) a_left = edge[n & 1][warp - 1];
             sp += mU;
-            if ((unsigned)(n - u) < width) {
+            if (MOD) {
+                // alpha(t,u) = lse(alpha(t-1,u) + lp_blank(t-1,u), alpha(t-1,u-1) + lp_label(t-1,u-1))
+                const P* slot = ring + rslot;   // this column's cell (n-1-u, u)
+                const bool prev_on = (unsigned)(n - 1 - u) < width;
+                const double left = u > 0 ? a_left : NINF;
+                const double stay = prev_on ? a + (double)slot[0].x : NINF;
+                const double a_prev = a;
+                if ((unsigned)(n - u) < width) {
+                    a = lse2<T>(stay, left);
+                    *sp = a;
+                } else if (n == last + 1 && u == Ub - 1) {
+                    ll_mod = lse2<T>(stay, left);   // the virtual cell (T, U-1)
+                }
+                off = prev_on && u < Ub - 1 ? a_prev + (double)slot[0].y : NINF;
+            } else if ((unsigned)(n - u) < width) {
                 const P* slot = ring + rslot;
                 const T sx = n > u ? slot[0].x : T(0);                   // lp_blank(t-1, u)
                 const T ey = u > 0 ? slot[-1].y : Real<T>::neg_inf();    // lp_label(t, u-1)
@@ -504,7 +527,7 @@ lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __rest
         }
         if (u == Ub - 1) {
             cp_async_wait<0>();
-            const double ll = a + (double)lp_u[(size_t)last * mU].x;
+            const double ll = MOD ? ll_mod : a + (double)lp_u[(size_t)last * mU].x;
             llf[b] = ll;
             costs[b] = (T)(-ll);
         }
@@ -525,10 +548,11 @@ lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __rest
             fslot = fslot >= (unsigned)NT ? fslot - NT : fslot + ring_elems - NT;
         }
         unsigned rslot = rstart;  // slot of diagonal n
+        double bprev = NINF;      // MOD: bv of one step earlier, beta(t+1,u+1) for the thread u-1
         for (int n = last; n >= 0; --n) {
             cp_async_wait<kRing - 2>();  // this thread's cell of diagonal n has landed
             if (MULTI) {
-                if (lane == 0) edge[n & 1][warp] = bv;
+                if (lane == 0) edge[n & 1][warp] = MOD ? bprev : bv;
                 __syncthreads();
             }
             // slot of diagonal n+1: written and read by this thread only
@@ -537,19 +561,41 @@ lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __rest
             gp -= mU;
             --fdg;
             fslot = fslot >= (unsigned)NT ? fslot - NT : fslot + ring_elems - NT;
-            double b_right = __shfl_down_sync(0xffffffffu, bv, 1);
+            double b_right = __shfl_down_sync(0xffffffffu, MOD ? bprev : bv, 1);
             if (MULTI && lane == 31 && warp + 1 < nwarps) b_right = edge[n & 1][warp + 1];
+            const double bold = bv;
             if ((unsigned)(n - u) < width) {
                 const P p = ring[rslot];
                 const T py = u < Ub - 1 ? p.y : Real<T>::neg_inf();
                 bv = lse2<T>(bv + (double)p.x, b_right + (double)py);
                 *sp = bv;
             }
+            if (MOD) bprev = bold;
             sp -= mU;
             rslot = rslot >= (unsigned)NT ? rslot - NT : rslot + ring_elems - NT;
         }
         if (u == 0) llb[b] = bv;
     }
+}
+template <typename T, bool MULTI>
+__global__ void __launch_bounds__(1024)
+lattice_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __restrict__ xlen,
+               const int* __restrict__ ylen, double* __restrict__ alphas,
+               double* __restrict__ betas, double* __restrict__ llf, double* __restrict__ llb,
+               T* __restrict__ costs, const Dims d) {
+    extern __shared__ __align__(16) unsigned char ring_raw[];
+    __shared__ double edge[2][32];
+    lattice_body<T, MULTI, false>(lp2, xlen, ylen, alphas, betas, llf, llb, costs, d, ring_raw, edge);
+}
+template <typename T, bool MULTI>
+__global__ void __launch_bounds__(1024)
+lattice_mod_kernel(const typename Real<T>::pair* __restrict__ lp2, const int* __restrict__ xlen,
+                   const int* __restrict__ ylen, double* __restrict__ alphas,
+                   double* __restrict__ betas, double* __restrict__ llf, double* __restrict__ llb,
+                   T* __restrict__ costs, const Dims d) {
+    extern __shared__ __align__(16) unsigned char ring_raw[];
+    __shared__ double edge[2][32];
+    lattice_body<T, MULTI, true>(lp2, xlen, ylen, alphas, betas, llf, llb, costs, d, ring_raw, edge);
 }
 
 // =================================================================================================
@@ -653,7 +699,10 @@ __device__ __forceinline__ VecT<T, VEC> grad_vec(const VecT<T, VEC>& x, const Ro
     }
     return g;
 }
+// MOD (the modified topology, DESIGN.md §11): the label term reads beta(t+1,u+1), and on the last frame exists
+// only at u = U-2, where beta(T,U-1) = 0; the blank term is the regular one.
 // fp64: lattices are natural-log doubles
+template <bool MOD = false>
 __device__ __forceinline__ RowGrad<double> row_grad_setup(const Dims& d, uint32_t r, uint32_t b, uint32_t t,
                                                           uint32_t u, int Tb, int Ub,
                                                           const int* __restrict__ labels,
@@ -676,13 +725,19 @@ __device__ __forceinline__ RowGrad<double> row_grad_setup(const Dims& d, uint32_
         g.cB = (occ - st.y) * R::kLog2e;
     g.y = -1;
     if ((int)u < Ub - 1) {
-        g.cL = ((occ + betas[q + d.maxU + 1]) - st.y) * R::kLog2e;
+        if (!MOD)
+            g.cL = ((occ + betas[q + d.maxU + 1]) - st.y) * R::kLog2e;
+        else if ((int)t < Tb - 1)
+            g.cL = ((occ + betas[q + 2 * d.maxU + 1]) - st.y) * R::kLog2e;
+        else if ((int)u == Ub - 2)
+            g.cL = (occ - st.y) * R::kLog2e;
         g.y = __ldg(labels + (size_t)b * (d.maxU - 1) + u);
     }
     return g;
 }
 // fp32: lattices are LogVal {e, log2 v}: the offsets are formed in the exp2 domain from an exact integer
 // part and a small float part - no conversions to double, no FP64 pipe
+template <bool MOD = false>
 __device__ __forceinline__ RowGrad<float> row_grad_setup(const Dims& d, uint32_t r, uint32_t b, uint32_t t,
                                                          uint32_t u, int Tb, int Ub,
                                                          const int* __restrict__ labels,
@@ -709,15 +764,23 @@ __device__ __forceinline__ RowGrad<float> row_grad_setup(const Dims& d, uint32_t
     }
     g.y = -1;
     if ((int)u < Ub - 1) {
-        const LogVal bn = betas[q + 1];
-        g.cL = (float)(oe + bn.e) + (ol + bn.l);
+        if (!MOD) {
+            const LogVal bn = betas[q + 1];
+            g.cL = (float)(oe + bn.e) + (ol + bn.l);
+        } else if ((int)t < Tb - 1) {
+            const LogVal bn = betas[q + d.maxU + 1];
+            g.cL = (float)(oe + bn.e) + (ol + bn.l);
+        } else if ((int)u == Ub - 2) {
+            g.cL = (float)oe + ol;
+        }
         g.y = __ldg(labels + (size_t)b * (d.maxU - 1) + u);
     }
     return g;
 }
 // Same constants with every load issued unconditionally and at once (short rows: the row's scalars are
 // the critical path of a chunk CTA, two dependent rounds of loads cost ~1 us).  Reads are in bounds for
-// every (t,u) of the tensor: q + maxU stays inside the lattice arrays plus the slack carve() leaves.
+// every (t,u) of the tensor: q + maxU (MOD: q + maxU + 1) stays inside the lattice arrays plus the slack carve() leaves.
+template <bool MOD = false>
 __device__ __forceinline__ RowGrad<float> row_grad_setup_spec(const Dims& d, uint32_t r, uint32_t b, uint32_t t,
                                                               uint32_t u, const int* __restrict__ xlen,
                                                               const int* __restrict__ ylen,
@@ -730,7 +793,7 @@ __device__ __forceinline__ RowGrad<float> row_grad_setup_spec(const Dims& d, uin
     const size_t q = cell(d, b, t, u);
     const int xl = __ldg(xlen + b), yl = __ldg(ylen + b);
     const float2 st = __ldg(stat + r);
-    const LogVal a = alphas[q], ll = llf[b], bq = betas[q], bt = betas[q + d.maxU], bu = betas[q + 1];
+    const LogVal a = alphas[q], ll = llf[b], bq = betas[q], bt = betas[q + d.maxU], bu = betas[q + (MOD ? d.maxU + 1 : 1)];
     const int lab = (int)u < d.maxU - 1 ? __ldg(labels + (size_t)b * (d.maxU - 1) + u) : 0;
     Tb = min(max(xl, 1), d.maxT);
     Ub = min(max(yl + 1, 1), d.maxU);
@@ -745,7 +808,8 @@ __device__ __forceinline__ RowGrad<float> row_grad_setup_spec(const Dims& d, uin
     g.cL = R::neg_inf();
     g.y = -1;
     if ((int)u < Ub - 1) {
-        g.cL = (float)(oe + bu.e) + (ol + bu.l);
+        if (!MOD || (int)t < Tb - 1) g.cL = (float)(oe + bu.e) + (ol + bu.l);
+        else if ((int)u == Ub - 2) g.cL = (float)oe + ol;
         g.y = lab;
     }
     return g;
@@ -760,7 +824,7 @@ __device__ __forceinline__ RowGrad<float> row_grad_setup_spec(const Dims& d, uin
 #ifndef RNNT_GRAD_MINB16
 #define RNNT_GRAD_MINB16 8   // 16-bit rows are one trip of 128 threads: residency (bytes in flight) is what pays
 #endif
-template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED, bool DELAY>
+template <typename T, int VEC, int NV, bool SCALED, typename IO, bool REG, bool PRUNED, bool DELAY, bool MOD = false>
 __device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __restrict__ grads,
                                          const int* __restrict__ labels, const int* __restrict__ xlen,
                                          const int* __restrict__ ylen, const typename Real<T>::pair* __restrict__ stat,
@@ -781,7 +845,8 @@ __device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __rest
     IO* grow = grads + (uint64_t)r * d.V;
     // per-utterance upstream gradient (autograd's grad_output) times the scalar factor
     const T scale = (SCALED && scale_vec) ? __ldg(scale_vec + b) * scale_in : scale_in;
-    if (PRUNED ? pruned_grad_padding(t, u, Tb, Ub, llf, b) : (int)t >= Tb || (int)u >= Ub) {
+    if (PRUNED ? pruned_grad_padding(t, u, Tb, Ub, llf, b)
+               : MOD ? mod_grad_padding(t, u, Tb, Ub, llf, b) : (int)t >= Tb || (int)u >= Ub) {
         VecT<T, VEC> z;
 #pragma unroll
         for (int c = 0; c < VEC; ++c) z.v[c] = 0;
@@ -800,7 +865,7 @@ __device__ __forceinline__ void grad_row(const IO* __restrict__ acts, IO* __rest
     };
     load(threadIdx.x);  // in flight before the lattice constants are fetched
     pdl_wait();         // (PDL) the logits were read ahead of the lattice kernel's completion; its output is not
-    RowGrad<T> rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
+    RowGrad<T> rg = row_grad_setup<MOD>(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
     if constexpr (REG) fastemit_fold(rg, reg, b, t, u, d);
     if constexpr (DELAY) delay_fold(rg, delay_log2, Tb, t);
     // 16-bit storage: fold the row maximum into the three offsets, one FFMA per element instead of FADD + FFMA
@@ -848,9 +913,23 @@ grad_row_delay_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const
     grad_row<T, VEC, NV, SCALED, IO, REG, PRUNED, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
                                                         scale_in, scale_vec, d, reg, p, delay_log2);
 }
+// The modified topology (DESIGN.md §11).  Its twins take the upstream scale, the gradient options and the delay
+// penalty as run-time values (scale 1, FastEmit off, clamp +inf and penalty 0 leave every value bitwise unchanged):
+// one instantiation per shape and PRUNED instead of sixteen keeps the library's compile time near the parent's.
+template <typename T, int VEC, int NV, typename IO, bool PRUNED>
+__global__ void __launch_bounds__(RowThreads<IO>::value, (sizeof(IO) >= 4 ? RNNT_GRAD_MINB : RNNT_GRAD_MINB16))
+grad_row_mod_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                    const int* __restrict__ xlen, const int* __restrict__ ylen,
+                    const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                    const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                    const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                    const Prune p, const T delay_log2) {
+    grad_row<T, VEC, NV, true, IO, true, PRUNED, true, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
+                                                             scale_in, scale_vec, d, reg, p, delay_log2);
+}
 
 // Pass 2, short rows: same register tile as rowstats_tile_kernel.
-template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED, bool DELAY>
+template <typename T, int VEC, int LPR, bool SCALED, typename IO, bool REG, bool PRUNED, bool DELAY, bool MOD = false>
 __device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __restrict__ grads,
                                           const int* __restrict__ labels, const int* __restrict__ xlen,
                                           const int* __restrict__ ylen, const typename Real<T>::pair* __restrict__ stat,
@@ -877,7 +956,8 @@ __device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __res
         const IO* row = acts + (uint64_t)r * d.V;
         IO* grow = grads + (uint64_t)r * d.V;
         const T scale = (SCALED && scale_vec) ? __ldg(scale_vec + b) * scale_in : scale_in;
-        if (PRUNED ? pruned_grad_padding(t, u, Tb, Ub, llf, b) : (int)t >= Tb || (int)u >= Ub) {
+        if (PRUNED ? pruned_grad_padding(t, u, Tb, Ub, llf, b)
+               : MOD ? mod_grad_padding(t, u, Tb, Ub, llf, b) : (int)t >= Tb || (int)u >= Ub) {
             VecT<T, VEC> z;
 #pragma unroll
             for (int c = 0; c < VEC; ++c) z.v[c] = 0;
@@ -895,7 +975,7 @@ __device__ __forceinline__ void grad_tile(const IO* __restrict__ acts, IO* __res
             if (i < nv) x[j] = ld_stream<T, VEC>(row + (size_t)i * VEC);
         }
         pdl_wait();
-        RowGrad<T> rg = row_grad_setup(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
+        RowGrad<T> rg = row_grad_setup<MOD>(d, r, b, t, u, Tb, Ub, labels, stat, alphas, betas, llf);
         if constexpr (REG) fastemit_fold(rg, reg, b, t, u, d);
         if constexpr (DELAY) delay_fold(rg, delay_log2, Tb, t);
 #pragma unroll
@@ -928,6 +1008,17 @@ grad_tile_delay_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, cons
                        const Prune p, const T delay_log2) {
     grad_tile<T, VEC, LPR, SCALED, IO, REG, PRUNED, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas, llf,
                                                           scale_in, scale_vec, d, reg, p, delay_log2);
+}
+template <typename T, int VEC, int LPR, typename IO, bool PRUNED>
+__global__ void __launch_bounds__(256)
+grad_tile_mod_kernel(const IO* __restrict__ acts, IO* __restrict__ grads, const int* __restrict__ labels,
+                     const int* __restrict__ xlen, const int* __restrict__ ylen,
+                     const typename Real<T>::pair* __restrict__ stat, const typename Lat<T>::val* __restrict__ alphas,
+                     const typename Lat<T>::val* __restrict__ betas, const typename Lat<T>::val* __restrict__ llf,
+                     const T scale_in, const T* __restrict__ scale_vec, const Dims d, const GradReg<T> reg,
+                     const Prune p, const T delay_log2) {
+    grad_tile<T, VEC, LPR, true, IO, true, PRUNED, true, true>(acts, grads, labels, xlen, ylen, stat, alphas, betas,
+                                                               llf, scale_in, scale_vec, d, reg, p, delay_log2);
 }
 
 }  // namespace b200rnnt

@@ -95,7 +95,12 @@ __device__ __forceinline__ void sts_volatile(uint32_t addr, int v) {
 // lane 33..64 labels are a single warp with no cross-warp exchange at all.
 // (See lattice_cols() for when that pays and when it does not.)
 // =================================================================================================
-template <int COLS, bool MULTI, bool BACKWARD, int RD>
+//
+// MOD: the modified topology (DESIGN.md §11), one transition per frame.  The label term of cell (t,u) comes from
+// (t-1,u-1) (alpha) / (t+1,u+1) (beta), which the neighbouring column held two diagonals before, so the offer
+// that crosses columns is the one of the previous step: ov2 / sv2 below, one step behind ov / sv.  Alpha runs one
+// diagonal further, to the virtual cell (T, U-1), whose value is the log-likelihood.
+template <int COLS, bool MULTI, bool BACKWARD, int RD, bool MOD = false>
 __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac, const int* __restrict__ xlen,
                                                  const int* __restrict__ ylen, LogVal* __restrict__ out,
                                                  LogVal* __restrict__ llout, float* __restrict__ costs,
@@ -116,7 +121,7 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
     int Tb, Ub;
     utt_extent(d, xlen, ylen, b, Tb, Ub);
     const size_t base = (size_t)b * lattice_block(d);
-    const int last = Tb + Ub - 2;
+    const int last = Tb + Ub - 2 + (MOD && !BACKWARD ? 1 : 0);
     const int mU = d.maxU;
     const int nactive = (Ub + 32 * COLS - 1) / (32 * COLS);   // warps that own at least one column
     if (MULTI && warp >= nactive) return;                     // no column of this warp exists in this utterance
@@ -144,8 +149,9 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
     int nu = n0 - u0;                                    // (current diagonal) - u0
     // Ring slots that no copy will fill hold NEUTRAL factors {1, 0, 1, log zero}: the step body below runs
     // unconditionally - a column that is not active yet keeps its "log zero" unchanged (and beta's virtual
-    // beta(T,U-1) = 1 in column U-1 cannot leak into column U-2), a column that has finished computes values
-    // nobody reads - and only the lattice STORE is predicated.
+    // beta(T,U-1) = 1 in column U-1 cannot leak into column U-2: in MOD it reaches U-2 one step later, through
+    // that column's own, real label factor of (T-1,U-2)), a column that has finished computes values nobody
+    // reads - and only the lattice STORE is predicated.
     auto neutral = [](uint32_t addr) {
         asm volatile("st.shared.v4.b32 [%0], {%1, %2, %1, %3};" ::"r"(addr), "r"(0x3f800000), "r"(0), "r"(kEZero) : "memory");
     };
@@ -166,12 +172,15 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
     uint32_t roff = 0;   // byte offset of the ring slot of step s0 (always 0 when the ring is one unroll group deep)
     // running values.  alpha: (sv,se) = alpha(t,u) p_blank(t,u) offered to (t+1,u), (ov,oe) = alpha(t,u)
     // p_label(t,u) offered to (t,u+1).  beta: (sv,se) = beta(t+1,u).
-    float sv[COLS], ov[COLS];
-    int se[COLS], oe[COLS];
+    // MOD: (ov2,oe2) / (sv2,se2) = the value (ov,oe) / (sv,se) had one step earlier.  (fv,fe) = alpha's virtual
+    // cell (T, U-1), taken from the last step.
+    float sv[COLS], ov[COLS], ov2[COLS], sv2[COLS], fv[COLS];
+    int se[COLS], oe[COLS], oe2[COLS], se2[COLS], fe[COLS];
 #pragma unroll
     for (int c = 0; c < COLS; ++c) {
         sv[c] = ov[c] = 1.0f;
         se[c] = oe[c] = kEZero;
+        if (MOD) sv2[c] = ov2[c] = fv[c] = 1.0f, se2[c] = oe2[c] = fe[c] = kEZero;
         if (!BACKWARD && u0 + c == 0) se[c] = 0;        // alpha(0,0) = 1 enters as the "stay" term of step 0
         if (BACKWARD && u0 + c == Ub - 1) se[c] = 0;    // virtual beta(T, U-1) = 1
     }
@@ -218,11 +227,11 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
             float nv;
             int ne;
             if (BACKWARD) {
-                nv = __shfl_down_sync(0xffffffffu, sv[0], 1);
-                ne = __shfl_down_sync(0xffffffffu, se[0], 1);
+                nv = __shfl_down_sync(0xffffffffu, MOD ? sv2[0] : sv[0], 1);
+                ne = __shfl_down_sync(0xffffffffu, MOD ? se2[0] : se[0], 1);
             } else {
-                nv = __shfl_up_sync(0xffffffffu, ov[COLS - 1], 1);
-                ne = __shfl_up_sync(0xffffffffu, oe[COLS - 1], 1);
+                nv = __shfl_up_sync(0xffffffffu, MOD ? ov2[COLS - 1] : ov[COLS - 1], 1);
+                ne = __shfl_up_sync(0xffffffffu, MOD ? oe2[COLS - 1] : oe[COLS - 1], 1);
             }
             if (MULTI && has_src) {
                 // value of step s-1 (tag s) from the neighbouring warp; at s == 0 nothing beside is active
@@ -238,25 +247,38 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
             if (BACKWARD) {
                 // beta(t,u) = beta(t+1,u) p_blank(t,u) + beta(t,u+1) p_label(t,u);  (t,u+1): the next column of
                 // this lane (previous step's value), or the next lane's first column for the last one
+                // (MOD: beta(t,u) = beta(t+1,u) p_blank(t,u) + beta(t+1,u+1) p_label(t,u), the next column's value
+                // of two steps ago)
 #pragma unroll
                 for (int c = 0; c < COLS; ++c) {
-                    const float rv = c + 1 < COLS ? sv[c + 1 < COLS ? c + 1 : c] : nv;
-                    const int re = c + 1 < COLS ? se[c + 1 < COLS ? c + 1 : c] : ne;
+                    const int cn = c + 1 < COLS ? c + 1 : c;
+                    const float rv = c + 1 < COLS ? (MOD ? sv2[cn] : sv[cn]) : nv;
+                    const int re = c + 1 < COLS ? (MOD ? se2[cn] : se[cn]) : ne;
                     lin_add(sv[c] * f[c].x, se[c] + __float_as_int(f[c].y), rv * f[c].z, re + __float_as_int(f[c].w), v[c], e[c]);
                 }
 #pragma unroll
-                for (int c = 0; c < COLS; ++c) sv[c] = v[c], se[c] = e[c];
+                for (int c = 0; c < COLS; ++c) {
+                    if (MOD) sv2[c] = sv[c], se2[c] = se[c];
+                    sv[c] = v[c], se[c] = e[c];
+                }
             } else {
                 // alpha(t,u) = [alpha(t-1,u) p_blank(t-1,u)] + [alpha(t,u-1) p_label(t,u-1)];  (t,u-1): the previous
                 // column of this lane (previous step's offer), or the previous lane's last column for the first one
+                // (MOD: alpha(t,u) = [alpha(t-1,u) p_blank(t-1,u)] + [alpha(t-1,u-1) p_label(t-1,u-1)], the previous
+                // column's offer of two steps ago)
 #pragma unroll
                 for (int c = 0; c < COLS; ++c) {
-                    const float lv = c > 0 ? ov[c > 0 ? c - 1 : 0] : nv;
-                    const int le = c > 0 ? oe[c > 0 ? c - 1 : 0] : ne;
+                    const int cp = c > 0 ? c - 1 : 0;
+                    const float lv = c > 0 ? (MOD ? ov2[cp] : ov[cp]) : nv;
+                    const int le = c > 0 ? (MOD ? oe2[cp] : oe[cp]) : ne;
                     lin_add(sv[c], se[c], lv, le, v[c], e[c]);
                 }
 #pragma unroll
                 for (int c = 0; c < COLS; ++c) {
+                    if (MOD) {
+                        ov2[c] = ov[c], oe2[c] = oe[c];
+                        if (s == last) fv[c] = v[c], fe[c] = e[c];   // the virtual cell (T, U-1) in column U-1
+                    }
                     sv[c] = v[c] * f[c].x, se[c] = e[c] + __float_as_int(f[c].y);   // offered to (t+1, u)
                     ov[c] = v[c] * f[c].z, oe[c] = e[c] + __float_as_int(f[c].w);   // offered to (t, u+1)
                 }
@@ -283,8 +305,8 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
             if (MULTI) {
                 const uint32_t slot_off = (eoff + (uint32_t)j * 16) & (kEdge * 16 - 1);
                 if (has_dst)
-                    edge_publish(my_edge + slot_off, BACKWARD ? sv[0] : ov[COLS - 1], BACKWARD ? se[0] : oe[COLS - 1], s + 1,
-                                 pub_lane);
+                    edge_publish(my_edge + slot_off, BACKWARD ? (MOD ? sv2[0] : sv[0]) : (MOD ? ov2[COLS - 1] : ov[COLS - 1]),
+                                 BACKWARD ? (MOD ? se2[0] : se[0]) : (MOD ? oe2[COLS - 1] : oe[COLS - 1]), s + 1, pub_lane);
                 if (has_src) {
                     sts_volatile(prog_base + warp * 4, s);   // every lane, same value: progress of this warp
                     pok = __all_sync(0xffffffffu, edge_read(src_edge + slot_off, s + 1, pv, pe));   // prefetch for the next step
@@ -321,16 +343,16 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
         bad = __any_sync(0xffffffffu, bad);
     }
     if (!BACKWARD) {
-        // (sv, se) of column U-1 = alpha(T-1,U-1) p_blank(T-1,U-1) after the last step
+        // (sv, se) of column U-1 = alpha(T-1,U-1) p_blank(T-1,U-1) after the last step (MOD: (fv, fe) = alpha(T,U-1))
         if ((Ub - 1) / COLS == tid) {
-            float fv = sv[0];
-            int fe = se[0];
+            float llv = MOD ? fv[0] : sv[0];
+            int lle = MOD ? fe[0] : se[0];
 #pragma unroll
             for (int c = 1; c < COLS; ++c)
-                if ((Ub - 1) % COLS == c) fv = sv[c], fe = se[c];
-            LogVal ll = to_logval(fv, fe);
+                if ((Ub - 1) % COLS == c) llv = MOD ? fv[c] : sv[c], lle = MOD ? fe[c] : se[c];
+            LogVal ll = to_logval(llv, lle);
             float cost = -(logval_log2(ll) * 0.6931471805599453f);
-            if (fe < kEDead) cost = INFINITY;
+            if (lle < kEDead) cost = INFINITY;
             if (bad) {
                 cost = __int_as_float(0x7fc00000);
                 ll.l = cost;
@@ -345,6 +367,29 @@ __device__ __forceinline__ void lattice_lin_body(const float4* __restrict__ fac,
     }
 }
 
+// The kernels' shared memory is declared in the kernels themselves (see rowstats_chunk_kernel) and handed in here.
+template <int COLS, bool MULTI, int RD, bool MOD>
+__device__ __forceinline__ void lattice_lin_run(const float4* __restrict__ fac, const int* __restrict__ xlen,
+                                                const int* __restrict__ ylen, LogVal* __restrict__ alphas,
+                                                LogVal* __restrict__ betas, LogVal* __restrict__ llf,
+                                                LogVal* __restrict__ llb, float* __restrict__ costs, const Dims& d,
+                                                unsigned char* ring_raw, int4* edge, int* prog, int* bad_any) {
+    if (MULTI) {
+        // tags start at 0 (= nothing published), progress at -1
+        for (int i = threadIdx.x; i < kEdgeWarps * kEdge; i += blockDim.x) edge[i] = make_int4(0, 0, 0, 0);
+        if (threadIdx.x < kEdgeWarps) prog[threadIdx.x] = -1;
+        if (threadIdx.x == 0) *bad_any = 0;
+        __syncthreads();
+    }
+    const uint32_t ring_base = smem_u32(ring_raw), edge_base = smem_u32(edge), prog_base = smem_u32(prog);
+    const uint32_t delay_base = ring_base + (uint32_t)RD * blockDim.x * COLS * 16u;   // MULTI only: [warps][8][32] x 8 B
+    pdl_trigger();   // the gradient kernel may launch and read the logits while the wavefront runs
+    pdl_wait();      // pass 1's factors are complete and visible
+    if (blockIdx.y == 0)
+        lattice_lin_body<COLS, MULTI, false, RD, MOD>(fac, xlen, ylen, alphas, llf, costs, d, ring_base, edge_base, prog_base, delay_base, bad_any);
+    else
+        lattice_lin_body<COLS, MULTI, true, RD, MOD>(fac, xlen, ylen, betas, llb, costs, d, ring_base, edge_base, prog_base, delay_base, bad_any);
+}
 template <int COLS, bool MULTI, int RD>
 __global__ void __launch_bounds__(MULTI ? 1024 / COLS : 32)
 lattice_lin_kernel(const float4* __restrict__ fac, const int* __restrict__ xlen, const int* __restrict__ ylen,
@@ -354,21 +399,21 @@ lattice_lin_kernel(const float4* __restrict__ fac, const int* __restrict__ xlen,
     __shared__ __align__(16) int4 edge[MULTI ? kEdgeWarps * kEdge : 1];
     __shared__ int prog[MULTI ? kEdgeWarps : 1];
     __shared__ int bad_any;
-    if (MULTI) {
-        // tags start at 0 (= nothing published), progress at -1
-        for (int i = threadIdx.x; i < kEdgeWarps * kEdge; i += blockDim.x) edge[i] = make_int4(0, 0, 0, 0);
-        if (threadIdx.x < kEdgeWarps) prog[threadIdx.x] = -1;
-        if (threadIdx.x == 0) bad_any = 0;
-        __syncthreads();
-    }
-    const uint32_t ring_base = smem_u32(ring_raw), edge_base = smem_u32(edge), prog_base = smem_u32(prog);
-    const uint32_t delay_base = ring_base + (uint32_t)RD * blockDim.x * COLS * 16u;   // MULTI only: [warps][8][32] x 8 B
-    pdl_trigger();   // the gradient kernel may launch and read the logits while the wavefront runs
-    pdl_wait();      // pass 1's factors are complete and visible
-    if (blockIdx.y == 0)
-        lattice_lin_body<COLS, MULTI, false, RD>(fac, xlen, ylen, alphas, llf, costs, d, ring_base, edge_base, prog_base, delay_base, &bad_any);
-    else
-        lattice_lin_body<COLS, MULTI, true, RD>(fac, xlen, ylen, betas, llb, costs, d, ring_base, edge_base, prog_base, delay_base, &bad_any);
+    lattice_lin_run<COLS, MULTI, RD, false>(fac, xlen, ylen, alphas, betas, llf, llb, costs, d, ring_raw, edge, prog,
+                                            &bad_any);
+}
+// the modified topology (DESIGN.md §11)
+template <int COLS, bool MULTI, int RD>
+__global__ void __launch_bounds__(MULTI ? 1024 / COLS : 32)
+lattice_lin_mod_kernel(const float4* __restrict__ fac, const int* __restrict__ xlen, const int* __restrict__ ylen,
+                       LogVal* __restrict__ alphas, LogVal* __restrict__ betas, LogVal* __restrict__ llf,
+                       LogVal* __restrict__ llb, float* __restrict__ costs, const Dims d) {
+    extern __shared__ __align__(16) unsigned char ring_raw[];
+    __shared__ __align__(16) int4 edge[MULTI ? kEdgeWarps * kEdge : 1];
+    __shared__ int prog[MULTI ? kEdgeWarps : 1];
+    __shared__ int bad_any;
+    lattice_lin_run<COLS, MULTI, RD, true>(fac, xlen, ylen, alphas, betas, llf, llb, costs, d, ring_raw, edge, prog,
+                                           &bad_any);
 }
 
 // Columns per lane for a label extent.  A lone warp issues about one instruction every few cycles whatever

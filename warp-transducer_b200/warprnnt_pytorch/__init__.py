@@ -4,8 +4,9 @@ Same public surface as the reference package (pytorch_binding/warprnnt_pytorch/_
 ``RNNTLoss(blank=0, reduction='mean')``, ``rnnt_loss(acts, labels, act_lens, label_lens,
 blank=0, reduction='mean')`` and the ``warp_rnnt`` extension functions, with the reference's
 input rules and error types (certify_inputs, :115-140).  Keyword-only additions:
-``fastemit_lambda`` (FastEmit regularisation), ``clamp`` (element-wise gradient clipping) and
-``delay_penalty`` (the delay-penalised lattice of low-latency streaming training); see rnnt_loss.  Differences, all on the fast side:
+``fastemit_lambda`` (FastEmit regularisation), ``clamp`` (element-wise gradient clipping),
+``delay_penalty`` (the delay-penalised lattice of low-latency streaming training) and ``rnnt_type``
+(k2's 'regular' or 'modified' one-symbol-per-frame topology); see rnnt_loss.  Differences, all on the fast side:
 the call never synchronises with the host except for the reference's own length check, costs
 stay on the device, and the gradient is produced in autograd's backward with grad_output and the
 'mean' factor folded into the kernel - no zeros_like / mul_ passes over the [N,T,U,V] tensor.
@@ -29,7 +30,7 @@ class _RNNT(Function):
 
     @staticmethod
     def forward(ctx, acts, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0, clamp=-1.0,
-                delay_penalty=0.0):
+                delay_penalty=0.0, rnnt_type='regular'):
         """
         acts: (batch x seqLength x labelLength x outputDim) raw joint-network logits
         labels: (batch x maxLabelLength) int32 targets, zero padded
@@ -37,6 +38,7 @@ class _RNNT(Function):
         """
         warp_rnnt.grad_options(fastemit_lambda, clamp)   # ValueError before any device work
         warp_rnnt.lattice_options(delay_penalty)
+        warp_rnnt.rnnt_type_code(rnnt_type)
         length_check = certify_inputs(acts, labels, act_lens, label_lens, defer=True)
         if not acts.is_cuda:
             raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only; "
@@ -50,13 +52,14 @@ class _RNNT(Function):
         # bf16 / fp16 logits: arithmetic, lattice and costs are fp32 (6 B per logit instead of 12)
         costs = torch.empty(minibatch_size, dtype=warp_rnnt.costs_dtype(acts), device=acts.device)
         ws = warp_rnnt.gpu_rnnt_forward(acts, labels, act_lens, label_lens, costs, blank,
-                                        prepare_backward=need_grad, delay_penalty=delay_penalty)
+                                        prepare_backward=need_grad, delay_penalty=delay_penalty, rnnt_type=rnnt_type)
         length_check.finish()   # T == max(act_lens), U == max(label_lens) + 1: waited for with the kernels queued
         if need_grad:
             ctx.save_for_backward(acts, labels, act_lens, label_lens)
             ctx.workspace = ws
             ctx.blank = blank
             ctx.fastemit_lambda, ctx.clamp, ctx.delay_penalty = fastemit_lambda, clamp, delay_penalty
+            ctx.rnnt_type = rnnt_type
             # reference :38-40 divides costs and grads by N for 'mean'
             ctx.scale = 1.0 / minibatch_size if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
@@ -75,12 +78,12 @@ class _RNNT(Function):
         grads = torch.empty_like(acts)   # the kernel defines every element (zeros on padding)
         warp_rnnt.gpu_rnnt_backward(acts, labels, act_lens, label_lens, grads, g, ctx.blank,
                                     ctx.scale, ctx.workspace, fastemit_lambda=ctx.fastemit_lambda,
-                                    clamp=ctx.clamp, delay_penalty=ctx.delay_penalty)
-        return grads, None, None, None, None, None, None, None, None
+                                    clamp=ctx.clamp, delay_penalty=ctx.delay_penalty, rnnt_type=ctx.rnnt_type)
+        return grads, None, None, None, None, None, None, None, None, None
 
 
 def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean', *, fastemit_lambda=0.0,
-              clamp=-1.0, delay_penalty=0.0):
+              clamp=-1.0, delay_penalty=0.0, rnnt_type='regular'):
     """RNN Transducer loss (reference :53-70).
 
     reduction: 'none' | 'sum' | 'mean'; 'mean' divides the summed loss by the batch size (what
@@ -97,28 +100,35 @@ def rnnt_loss(acts, labels, act_lens, label_lens, blank=0, reduction='mean', *, 
     >= 0; 0 = off.  Every label factor at frame t gains delay_penalty * ((T_b - 1)/2 - t), T_b the utterance's
     frame count; the returned loss includes the penalty (it can be negative) and the gradient is its exact
     gradient.  It favours emitting labels early (include/rnnt.h, rnntLatticeOptions).
+    rnnt_type: 'regular' (default) or 'modified', k2's one-symbol-per-frame transducer: every frame takes exactly
+    one transition, a blank or the next label, so a frame emits at most one label.  An utterance with more labels
+    than frames then has no path: its loss is +inf and its gradient zero.  'constrained' is not supported.
     Invalid values raise ValueError.
     """
-    return _RNNT.apply(acts, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, clamp, delay_penalty)
+    return _RNNT.apply(acts, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, clamp, delay_penalty,
+                       rnnt_type)
 
 
 class RNNTLoss(Module):
     """Module form (reference :73-100): RNNTLoss(blank=0, reduction='mean', *, fastemit_lambda=0.0,
-    clamp=-1.0, delay_penalty=0.0); the keyword-only options are those of rnnt_loss."""
+    clamp=-1.0, delay_penalty=0.0, rnnt_type='regular'); the keyword-only options are those of rnnt_loss."""
 
-    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0,
+                 rnnt_type='regular'):
         super(RNNTLoss, self).__init__()
         warp_rnnt.grad_options(fastemit_lambda, clamp)
         warp_rnnt.lattice_options(delay_penalty)
+        warp_rnnt.rnnt_type_code(rnnt_type)
         self.blank = blank
         self.reduction = reduction
         self.fastemit_lambda, self.clamp = fastemit_lambda, clamp
         self.delay_penalty = delay_penalty
+        self.rnnt_type = rnnt_type
         self.loss = _RNNT.apply
 
     def forward(self, acts, labels, act_lens, label_lens):
         return self.loss(acts, labels, act_lens, label_lens, self.blank, self.reduction, self.fastemit_lambda,
-                         self.clamp, self.delay_penalty)
+                         self.clamp, self.delay_penalty, self.rnnt_type)
 
 
 from ._checks import certify_inputs, check_contiguous, check_dim, check_type  # noqa: E402,F401

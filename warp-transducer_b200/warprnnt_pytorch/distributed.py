@@ -9,7 +9,7 @@ import torch
 import torch.distributed as dist
 
 from . import _RNNT, certify_inputs  # noqa: F401
-from .warp_rnnt import grad_options, lattice_options
+from .warp_rnnt import grad_options, lattice_options, rnnt_type_code
 
 
 def shard_bounds(n_global, rank, world):
@@ -45,13 +45,16 @@ class ShardedRNNTLoss(torch.nn.Module):
     local shard.  n_global must be known up front for 'mean' (it fixes the gradient scale before
     the collective completes, so no host synchronisation is needed); pass None to infer it as
     world_size * local batch.  fastemit_lambda / clamp: the keyword-only gradient options of rnnt_loss; the
-    clip applies to each utterance's gradient before the 1/N_global of 'mean'.  delay_penalty: rnnt_loss's."""
+    clip applies to each utterance's gradient before the 1/N_global of 'mean'.  delay_penalty and rnnt_type:
+    rnnt_loss's."""
 
     def __init__(self, blank=0, reduction='mean', group=None, n_global=None, *, fastemit_lambda=0.0, clamp=-1.0,
-                 delay_penalty=0.0):
+                 delay_penalty=0.0, rnnt_type='regular'):
         super().__init__()
         grad_options(fastemit_lambda, clamp)
         lattice_options(delay_penalty)
+        rnnt_type_code(rnnt_type)
+        self.rnnt_type = rnnt_type
         self.blank, self.reduction, self.group, self.n_global = blank, reduction, group, n_global
         self.fastemit_lambda, self.clamp = fastemit_lambda, clamp
         self.delay_penalty = delay_penalty
@@ -61,7 +64,7 @@ class ShardedRNNTLoss(torch.nn.Module):
         n_local = acts.size(0)
         n_global = self.n_global if self.n_global is not None else n_local * world
         local = _RNNT.apply(acts, labels, act_lens, label_lens, self.blank, 'sum', self.fastemit_lambda,
-                            self.clamp, self.delay_penalty)   # [1], grads unscaled
+                            self.clamp, self.delay_penalty, self.rnnt_type)   # [1], grads unscaled
         if self.reduction == 'mean':
             local = local / n_global            # autograd carries the 1/N_global into backward
         if world > 1:

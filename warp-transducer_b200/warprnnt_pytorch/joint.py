@@ -17,6 +17,8 @@ c = 1 - lm_only_scale - am_only_scale (include/rnnt.h, rnntSmoothOptions; DESIGN
 
 The keyword-only ``delay_penalty`` is RNNTLoss's: each label factor at frame t gains delay_penalty * ((T_b - 1)/2 - t),
 added after the smoothing interpolation (DESIGN.md §10); the loss includes it and the gradients are exact.
+
+The keyword-only ``rnnt_type`` is RNNTLoss's: 'regular' or 'modified' (one symbol per frame, DESIGN.md §11).
 """
 import ctypes as C
 import math
@@ -64,6 +66,14 @@ _lib.rnnt_b200_add_joint_smoothed_backward.restype = C.c_int
 _lib.rnnt_b200_add_joint_smoothed_backward.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_float,
                                                        warp_rnnt.rnntGradOptions, rnntSmoothOptions, _P,
                                                        warp_rnnt.rnntOptions]
+_lib.rnnt_b200_add_joint_forward_topo.restype = C.c_int
+_lib.rnnt_b200_add_joint_forward_topo.argtypes = [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int,
+                                                  rnntSmoothOptions, warp_rnnt.rnntLatticeOptions, C.c_int, _P,
+                                                  warp_rnnt.rnntOptions]
+_lib.rnnt_b200_add_joint_backward_topo.restype = C.c_int
+_lib.rnnt_b200_add_joint_backward_topo.argtypes = [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_float,
+                                                   warp_rnnt.rnntGradOptions, rnntSmoothOptions, C.c_int, _P,
+                                                   warp_rnnt.rnntOptions]
 
 
 def smooth_options(lm_only_scale=0.0, am_only_scale=0.0):
@@ -135,10 +145,12 @@ def _joint_opts(trans, pred, blank):
 _lab_ptr = warp_rnnt._labels_ptr   # cached per-device stand-in when there are no labels (U == 1)
 
 
-def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare_backward, blank, smooth, lattice=None):
+def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare_backward, blank, smooth, lattice=None,
+                       topo=warp_rnnt.RNNT_B200_RNNT_REGULAR):
     """The forward half on CUDA tensors (no checks): rnnt_b200_add_joint_forward, or its smoothed form when
     `smooth` (an rnntSmoothOptions) is given, or rnnt_b200_add_joint_forward_lat when `lattice` (an
-    rnntLatticeOptions) is given.  Returns the workspace the backward half and the ranges read."""
+    rnntLatticeOptions) is given, or rnnt_b200_add_joint_forward_topo for the modified topology `topo`.  Returns
+    the workspace the backward half and the ranges read."""
     N, T, V = trans.shape
     U = pred.shape[1]
     n = C.c_size_t(0)
@@ -150,7 +162,11 @@ def joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, prepare
     args = (trans.data_ptr(), pred.data_ptr(), _lab_ptr(labels), label_lens.data_ptr(), act_lens.data_ptr(), V, N,
             costs.data_ptr(), 1 if prepare_backward else 0)
     tail = (ws.data_ptr(), _joint_opts(trans, pred, blank))
-    if lattice is not None:
+    if topo != warp_rnnt.RNNT_B200_RNNT_REGULAR:
+        st = _lib.rnnt_b200_add_joint_forward_topo(*args, smooth if smooth is not None else rnntSmoothOptions(),
+                                                   lattice if lattice is not None else warp_rnnt.rnntLatticeOptions(),
+                                                   topo, *tail)
+    elif lattice is not None:
         st = _lib.rnnt_b200_add_joint_forward_lat(*args, smooth if smooth is not None else rnntSmoothOptions(),
                                                   lattice, *tail)
     elif smooth is None:
@@ -185,8 +201,9 @@ class _AddJointRNNT(Function):
 
     @staticmethod
     def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda=0.0,
-                lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
+                lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0, rnnt_type='regular'):
         lattice = warp_rnnt.lattice_options(delay_penalty)   # ValueError before any device work
+        topo = warp_rnnt.rnnt_type_code(rnnt_type)
         gopt, smooth, length_check = check_joint_call(trans, pred, labels, act_lens, label_lens, reduction,
                                                       fastemit_lambda, lm_only_scale, am_only_scale)
         N = trans.shape[0]
@@ -194,11 +211,12 @@ class _AddJointRNNT(Function):
         need = trans.requires_grad or pred.requires_grad
         costs = torch.empty(N, dtype=torch.float32, device=trans.device)
         with torch.cuda.device(trans.device):
-            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, need, blank, smooth, lattice)
+            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, need, blank, smooth, lattice,
+                                    topo)
         length_check.finish()   # the reference's length test, waited for with the kernels already queued
         if need:
             ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
-            ctx.ws, ctx.blank, ctx.gopt, ctx.smooth = ws, blank, gopt, smooth
+            ctx.ws, ctx.blank, ctx.gopt, ctx.smooth, ctx.topo = ws, blank, gopt, smooth, topo
             ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -217,7 +235,11 @@ class _AddJointRNNT(Function):
             args = (trans.data_ptr(), pred.data_ptr(), dtrans.data_ptr(), dpred.data_ptr(), _lab_ptr(labels),
                     label_lens.data_ptr(), act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale)
             tail = (ctx.ws.data_ptr(), _joint_opts(trans, pred, ctx.blank))
-            if ctx.smooth is not None:
+            if ctx.topo != warp_rnnt.RNNT_B200_RNNT_REGULAR:
+                st = _lib.rnnt_b200_add_joint_backward_topo(
+                    *args, warp_rnnt.rnntGradOptions() if ctx.gopt is None else ctx.gopt,
+                    rnntSmoothOptions() if ctx.smooth is None else ctx.smooth, ctx.topo, *tail)
+            elif ctx.smooth is not None:
                 gopt = warp_rnnt.rnntGradOptions() if ctx.gopt is None else ctx.gopt
                 st = _lib.rnnt_b200_add_joint_smoothed_backward(*args, gopt, ctx.smooth, *tail)
             elif ctx.gopt is not None:
@@ -226,7 +248,7 @@ class _AddJointRNNT(Function):
                 st = _lib.rnnt_b200_add_joint_backward(*args, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_add_joint_backward failed: " + warp_rnnt.status_string(st))
-        return dtrans, dpred, None, None, None, None, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None, None, None, None, None
 
 
 def _no_clamp(clamp):
@@ -236,27 +258,30 @@ def _no_clamp(clamp):
 
 
 def add_joint_rnnt_loss(trans, pred, labels, act_lens, label_lens, blank=0, reduction='mean', *,
-                        fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
+                        fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0,
+                        rnnt_type='regular'):
     """fastemit_lambda: as rnnt_loss (the gradient is then not the gradient of the returned loss).
     lm_only_scale, am_only_scale: the smoothed loss (module docstring); both 0 is the plain loss.
-    delay_penalty: as rnnt_loss, added after the smoothing (module docstring)."""
+    delay_penalty: as rnnt_loss, added after the smoothing (module docstring).  rnnt_type: as rnnt_loss."""
     _no_clamp(clamp)
     return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
-                               lm_only_scale, am_only_scale, delay_penalty)
+                               lm_only_scale, am_only_scale, delay_penalty, rnnt_type)
 
 
 class AddJointRNNTLoss(Module):
     def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=None, lm_only_scale=0.0,
-                 am_only_scale=0.0, delay_penalty=0.0):
+                 am_only_scale=0.0, delay_penalty=0.0, rnnt_type='regular'):
         super().__init__()
         _no_clamp(clamp)
         warp_rnnt.grad_options(fastemit_lambda)
         smooth_options(lm_only_scale, am_only_scale)
         warp_rnnt.lattice_options(delay_penalty)
+        warp_rnnt.rnnt_type_code(rnnt_type)
         self.blank, self.reduction, self.fastemit_lambda = blank, reduction, fastemit_lambda
         self.lm_only_scale, self.am_only_scale = lm_only_scale, am_only_scale
-        self.delay_penalty = delay_penalty
+        self.delay_penalty, self.rnnt_type = delay_penalty, rnnt_type
 
     def forward(self, trans, pred, labels, act_lens, label_lens):
         return _AddJointRNNT.apply(trans, pred, labels, act_lens, label_lens, self.blank, self.reduction,
-                                   self.fastemit_lambda, self.lm_only_scale, self.am_only_scale, self.delay_penalty)
+                                   self.fastemit_lambda, self.lm_only_scale, self.am_only_scale, self.delay_penalty,
+                                   self.rnnt_type)

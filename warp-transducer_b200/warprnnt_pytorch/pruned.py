@@ -47,8 +47,19 @@ _lib.rnnt_b200_pruned_backward_lat.argtypes = [C.c_int, _P, _P, _P, C.c_int, _P,
 _lib.rnnt_b200_pruned_loss_async_lat.restype = C.c_int
 _lib.rnnt_b200_pruned_loss_async_lat.argtypes = [C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int,
                                                  C.c_int, _P, C.c_double, _GOpt, _LOpt, _P, _Opt]
+_lib.rnnt_b200_pruned_forward_topo.restype = C.c_int
+_lib.rnnt_b200_pruned_forward_topo.argtypes = [C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int,
+                                               _LOpt, C.c_int, _P, _Opt]
+_lib.rnnt_b200_pruned_backward_topo.restype = C.c_int
+_lib.rnnt_b200_pruned_backward_topo.argtypes = [C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P,
+                                                C.c_double, _GOpt, _LOpt, C.c_int, _P, _Opt]
+_lib.rnnt_b200_pruned_loss_async_topo.restype = C.c_int
+_lib.rnnt_b200_pruned_loss_async_topo.argtypes = [C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, C.c_int,
+                                                  C.c_int, _P, C.c_double, _GOpt, _LOpt, C.c_int, _P, _Opt]
 _lib.rnnt_b200_add_joint_prune_ranges.restype = C.c_int
 _lib.rnnt_b200_add_joint_prune_ranges.argtypes = [_P, _P, C.c_int, C.c_int, _P, _P, _Opt]
+_lib.rnnt_b200_add_joint_prune_ranges_topo.restype = C.c_int
+_lib.rnnt_b200_add_joint_prune_ranges_topo.argtypes = [_P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _Opt]
 _lib.rnnt_b200_add_joint_workspace_size.restype = C.c_int
 
 
@@ -66,11 +77,12 @@ class _AddJointRNNTRanges(Function):
 
     @staticmethod
     def forward(ctx, trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda, s_range,
-                lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
+                lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0, rnnt_type='regular'):
         s_range = int(s_range)
         if s_range < 2:
             raise ValueError("s_range must be >= 2, got %d" % s_range)
         lattice = warp_rnnt.lattice_options(delay_penalty)
+        topo = warp_rnnt.rnnt_type_code(rnnt_type)
         gopt, smooth, length_check = check_joint_call(trans, pred, labels, act_lens, label_lens, reduction,
                                                       fastemit_lambda, lm_only_scale, am_only_scale)
         N, T = trans.shape[0], trans.shape[1]
@@ -78,16 +90,22 @@ class _AddJointRNNTRanges(Function):
         costs = torch.empty(N, dtype=torch.float32, device=trans.device)
         ranges = torch.empty((N, T), dtype=torch.int32, device=trans.device)
         with torch.cuda.device(trans.device):
-            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, True, blank, smooth, lattice)
-            st = _lib.rnnt_b200_add_joint_prune_ranges(label_lens.data_ptr(), act_lens.data_ptr(), N, s_range,
-                                                       ranges.data_ptr(), ws.data_ptr(),
-                                                       _joint_opts(trans, pred, blank))
+            ws = joint_forward_call(trans, pred, labels, act_lens, label_lens, costs, True, blank, smooth, lattice,
+                                    topo)
+            if topo != warp_rnnt.RNNT_B200_RNNT_REGULAR:
+                st = _lib.rnnt_b200_add_joint_prune_ranges_topo(label_lens.data_ptr(), act_lens.data_ptr(), N,
+                                                                s_range, ranges.data_ptr(), ws.data_ptr(), topo,
+                                                                _joint_opts(trans, pred, blank))
+            else:
+                st = _lib.rnnt_b200_add_joint_prune_ranges(label_lens.data_ptr(), act_lens.data_ptr(), N, s_range,
+                                                           ranges.data_ptr(), ws.data_ptr(),
+                                                           _joint_opts(trans, pred, blank))
         if st != 0:
             raise RuntimeError("rnnt_b200_add_joint_prune_ranges failed: " + warp_rnnt.status_string(st))
         length_check.finish()
         ctx.mark_non_differentiable(ranges)
         ctx.save_for_backward(trans, pred, labels, act_lens, label_lens)
-        ctx.ws, ctx.blank, ctx.gopt, ctx.smooth = ws, blank, gopt, smooth
+        ctx.ws, ctx.blank, ctx.gopt, ctx.smooth, ctx.topo = ws, blank, gopt, smooth, topo
         ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -98,19 +116,22 @@ class _AddJointRNNTRanges(Function):
     @staticmethod
     def backward(ctx, grad_output, grad_ranges):
         dtrans, dpred = _AddJointRNNT.backward(ctx, grad_output)[:2]
-        return dtrans, dpred, None, None, None, None, None, None, None, None, None, None
+        return dtrans, dpred, None, None, None, None, None, None, None, None, None, None, None
 
 
 def add_joint_rnnt_loss_with_ranges(trans, pred, labels, act_lens, label_lens, s_range, blank=0, reduction='mean',
-                                    *, fastemit_lambda=0.0, lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0):
+                                    *, fastemit_lambda=0.0, lm_only_scale=0.0, am_only_scale=0.0, delay_penalty=0.0,
+                                    rnnt_type='regular'):
     """(loss, ranges): add_joint_rnnt_loss (the "simple" loss of pruned RNN-T; differentiable in trans and pred
     exactly as add_joint_rnnt_loss) and the [N, T] int32 window starts of the pruned loss for R = s_range >= 2,
     from the same forward (include/rnnt.h, rnnt_b200_add_joint_prune_ranges, defines them).  lm_only_scale and
     am_only_scale smooth the simple loss as add_joint_rnnt_loss's do (icefall's --lm-scale / --am-scale); the
     windows then come from the smoothed lattice.  delay_penalty penalises it as add_joint_rnnt_loss's does (icefall's
-    --delay-penalty), and the windows come from the penalised lattice, as k2's do."""
+    --delay-penalty), and the windows come from the penalised lattice, as k2's do.  rnnt_type: rnnt_loss's; the
+    windows of a 'modified' lattice come from its own occupancies and may leave an utterance no path through the
+    pruned modified loss (DESIGN.md §11)."""
     return _AddJointRNNTRanges.apply(trans, pred, labels, act_lens, label_lens, blank, reduction, fastemit_lambda,
-                                     s_range, lm_only_scale, am_only_scale, delay_penalty)
+                                     s_range, lm_only_scale, am_only_scale, delay_penalty, rnnt_type)
 
 
 def prune_joint_inputs(enc, dec, ranges, s_range):
@@ -164,9 +185,10 @@ class _PrunedRNNT(Function):
 
     @staticmethod
     def forward(ctx, logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda=0.0,
-                clamp=-1.0, delay_penalty=0.0):
+                clamp=-1.0, delay_penalty=0.0, rnnt_type='regular'):
         warp_rnnt.grad_options(fastemit_lambda, clamp)   # ValueError before any device work
         lattice = warp_rnnt.lattice_options(delay_penalty)
+        topo = warp_rnnt.rnnt_type_code(rnnt_type)
         code = warp_rnnt._dtype_code(logits)
         if reduction not in ('none', 'sum', 'mean'):
             raise ValueError("reduction must be 'none', 'sum' or 'mean'")
@@ -182,7 +204,9 @@ class _PrunedRNNT(Function):
             args = (code, logits.data_ptr(), ranges.data_ptr(), R, _lab_ptr(labels), label_lens.data_ptr(),
                     act_lens.data_ptr(), V, N, costs.data_ptr(), 1 if need_grad else 0)
             tail = (ws.data_ptr(), _opts(logits, blank, U))
-            if lattice is None:
+            if topo != warp_rnnt.RNNT_B200_RNNT_REGULAR:
+                st = _lib.rnnt_b200_pruned_forward_topo(*args, lattice or _LOpt(), topo, *tail)
+            elif lattice is None:
                 st = _lib.rnnt_b200_pruned_forward(*args, *tail)
             else:
                 st = _lib.rnnt_b200_pruned_forward_lat(*args, lattice, *tail)
@@ -192,7 +216,7 @@ class _PrunedRNNT(Function):
         if need_grad:
             ctx.save_for_backward(logits, labels, act_lens, label_lens, ranges)
             ctx.workspace, ctx.blank, ctx.maxU = ws, blank, U
-            ctx.fastemit_lambda, ctx.clamp, ctx.lattice = fastemit_lambda, clamp, lattice
+            ctx.fastemit_lambda, ctx.clamp, ctx.lattice, ctx.topo = fastemit_lambda, clamp, lattice, topo
             ctx.scale = 1.0 / N if reduction == 'mean' else 1.0
         if reduction in ('sum', 'mean'):
             costs = costs.sum().unsqueeze_(-1)
@@ -212,37 +236,43 @@ class _PrunedRNNT(Function):
             args = (warp_rnnt._dtype_code(logits), logits.data_ptr(), grads.data_ptr(), ranges.data_ptr(), R,
                     _lab_ptr(labels), label_lens.data_ptr(), act_lens.data_ptr(), V, N, g.data_ptr(), ctx.scale, gopt)
             tail = (ctx.workspace.data_ptr(), _opts(logits, ctx.blank, ctx.maxU))
-            if ctx.lattice is None:
+            if ctx.topo != warp_rnnt.RNNT_B200_RNNT_REGULAR:
+                st = _lib.rnnt_b200_pruned_backward_topo(*args, ctx.lattice or _LOpt(), ctx.topo, *tail)
+            elif ctx.lattice is None:
                 st = _lib.rnnt_b200_pruned_backward_ex(*args, *tail)
             else:
                 st = _lib.rnnt_b200_pruned_backward_lat(*args, ctx.lattice, *tail)
         if st != 0:
             raise RuntimeError("rnnt_b200_pruned_backward_ex failed: " + warp_rnnt.status_string(st))
-        return grads, None, None, None, None, None, None, None, None, None
+        return grads, None, None, None, None, None, None, None, None, None, None
 
 
 def pruned_rnnt_loss(logits, labels, act_lens, label_lens, ranges, blank=0, reduction='mean', *,
-                     fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
+                     fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0, rnnt_type='regular'):
     """Pruned RNN-T loss of logits [N, T, R, V] (fp32 / fp64 / bf16 / fp16), row (b, t, s) = lattice cell
     (t, ranges[b, t] + s); ranges [N, T] int32 on the logits' device.  labels, lengths, reduction and the gradient
     options are rnnt_loss's; the lattice is [T, max(label_lens) + 1] as there.  An utterance whose windows leave no
     path costs +inf with a zero gradient.  With R = U and ranges == 0 this is rnnt_loss exactly.  delay_penalty:
-    rnnt_loss's, on the covered cells (icefall passes the same value to the simple and the pruned loss)."""
+    rnnt_loss's, on the covered cells (icefall passes the same value to the simple and the pruned loss).
+    rnnt_type: rnnt_loss's; with 'modified' the windows may leave an utterance no path (DESIGN.md §11)."""
     return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, blank, reduction, fastemit_lambda, clamp,
-                             delay_penalty)
+                             delay_penalty, rnnt_type)
 
 
 class PrunedRNNTLoss(Module):
     """Module form of pruned_rnnt_loss: PrunedRNNTLoss(blank=0, reduction='mean', *, fastemit_lambda=0.0,
-    clamp=-1.0, delay_penalty=0.0)(logits, labels, act_lens, label_lens, ranges)."""
+    clamp=-1.0, delay_penalty=0.0, rnnt_type='regular')(logits, labels, act_lens, label_lens, ranges)."""
 
-    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
+    def __init__(self, blank=0, reduction='mean', *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0,
+                 rnnt_type='regular'):
         super().__init__()
         warp_rnnt.grad_options(fastemit_lambda, clamp)
         warp_rnnt.lattice_options(delay_penalty)
+        warp_rnnt.rnnt_type_code(rnnt_type)
         self.blank, self.reduction = blank, reduction
         self.fastemit_lambda, self.clamp, self.delay_penalty = fastemit_lambda, clamp, delay_penalty
+        self.rnnt_type = rnnt_type
 
     def forward(self, logits, labels, act_lens, label_lens, ranges):
         return _PrunedRNNT.apply(logits, labels, act_lens, label_lens, ranges, self.blank, self.reduction,
-                                 self.fastemit_lambda, self.clamp, self.delay_penalty)
+                                 self.fastemit_lambda, self.clamp, self.delay_penalty, self.rnnt_type)

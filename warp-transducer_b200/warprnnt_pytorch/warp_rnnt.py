@@ -89,6 +89,16 @@ _lib.rnnt_b200_forward_lat.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int
 _lib.rnnt_b200_backward_lat.restype = C.c_int
 _lib.rnnt_b200_backward_lat.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
                                         rnntGradOptions, rnntLatticeOptions, _P, rnntOptions]
+RNNT_B200_RNNT_REGULAR, RNNT_B200_RNNT_MODIFIED = 0, 1
+_lib.rnnt_b200_loss_async_topo.restype = C.c_int
+_lib.rnnt_b200_loss_async_topo.argtypes = [C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
+                                           rnntGradOptions, rnntLatticeOptions, C.c_int, _P, rnntOptions]
+_lib.rnnt_b200_forward_topo.restype = C.c_int
+_lib.rnnt_b200_forward_topo.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, rnntLatticeOptions,
+                                        C.c_int, _P, rnntOptions]
+_lib.rnnt_b200_backward_topo.restype = C.c_int
+_lib.rnnt_b200_backward_topo.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
+                                         rnntGradOptions, rnntLatticeOptions, C.c_int, _P, rnntOptions]
 _lib.get_workspace_size.restype = C.c_int
 _lib.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
 _lib.get_warprnnt_version.restype = C.c_int
@@ -229,6 +239,20 @@ def lattice_options(delay_penalty=0.0):
     return None if lam == 0.0 else rnntLatticeOptions(lam)
 
 
+_RNNT_TYPES = {'regular': RNNT_B200_RNNT_REGULAR, 'modified': RNNT_B200_RNNT_MODIFIED}
+
+
+def rnnt_type_code(rnnt_type):
+    """The C-ABI's rnnt_type for k2's `rnnt_type` name: 'regular' (any number of labels per frame) or 'modified'
+    (at most one symbol per frame, include/rnnt.h RNNT_B200_RNNT_MODIFIED).  Anything else raises ValueError,
+    k2's 'constrained' included."""
+    if rnnt_type == 'constrained':
+        raise ValueError("rnnt_type='constrained' is not supported; use 'regular' or 'modified'")
+    if not isinstance(rnnt_type, str) or rnnt_type not in _RNNT_TYPES:
+        raise ValueError("rnnt_type must be 'regular' or 'modified', got %r" % (rnnt_type,))
+    return _RNNT_TYPES[rnnt_type]
+
+
 def _dtype_code(acts):
     code = {torch.float32: RNNT_B200_FP32, torch.float64: RNNT_B200_FP64, torch.bfloat16: RNNT_B200_BF16,
             torch.float16: RNNT_B200_FP16}.get(acts.dtype)
@@ -252,9 +276,10 @@ def _workspace(acts, T, U, N, workspace):
 
 
 def _loss_async(layout, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                grad_scale, workspace, fastemit_lambda, clamp, delay_penalty=0.0):
+                grad_scale, workspace, fastemit_lambda, clamp, delay_penalty=0.0, rnnt_type='regular'):
     gopt = _ex_options(fastemit_lambda, clamp)
     lopt = lattice_options(delay_penalty)
+    topo = rnnt_type_code(rnnt_type)
     code = _dtype_code(acts)
     if layout == RNNT_B200_LAYOUT_TUNV and code not in (RNNT_B200_FP32, RNNT_B200_FP64):
         raise TypeError("unsupported data type %s for the time-major layout" % acts.dtype)
@@ -264,7 +289,9 @@ def _loss_async(layout, T, U, N, V, acts, labels, input_lengths, label_lengths, 
         opt.maxT, opt.maxU = T, U
         args = (code, layout, acts.data_ptr(), _ptr(grads), _labels_ptr(labels), label_lengths.data_ptr(),
                 input_lengths.data_ptr(), V, N, costs.data_ptr(), grad_scale, gopt)
-        if lopt is None:
+        if topo != RNNT_B200_RNNT_REGULAR:
+            st = _lib.rnnt_b200_loss_async_topo(*args, lopt or rnntLatticeOptions(), topo, workspace.data_ptr(), opt)
+        elif lopt is None:
             st = _lib.rnnt_b200_loss_async_ex(*args, workspace.data_ptr(), opt)
         else:
             st = _lib.rnnt_b200_loss_async_lat(*args, lopt, workspace.data_ptr(), opt)
@@ -274,26 +301,28 @@ def _loss_async(layout, T, U, N, V, acts, labels, input_lengths, label_lengths, 
 
 
 def gpu_rnnt_async(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                   grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
+                   grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0,
+                   rnnt_type='regular'):
     """Extension: no host synchronisation, `costs` on the device, gradients pre-multiplied by
     `grad_scale`.  Returns the workspace tensor (keep it alive until the stream has run).
     fastemit_lambda / clamp: gradient options (see grad_options); the costs do not depend on them, and
     with FastEmit on the gradient is not the gradient of the costs.  delay_penalty: the lattice option (see
-    lattice_options); it changes the costs and the gradient."""
+    lattice_options); it changes the costs and the gradient.  rnnt_type: the topology (see rnnt_type_code)."""
     N, T, U, V = acts.shape
     return _loss_async(RNNT_B200_LAYOUT_NTUV, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads,
-                       blank_label, grad_scale, workspace, fastemit_lambda, clamp, delay_penalty)
+                       blank_label, grad_scale, workspace, fastemit_lambda, clamp, delay_penalty, rnnt_type)
 
 
 def gpu_rnnt_async_tunv(acts, labels, input_lengths, label_lengths, costs, grads, blank_label,
-                        grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
+                        grad_scale=1.0, workspace=None, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0,
+                        rnnt_type='regular'):
     """Time-major extension: `acts` / `grads` are [T, U, N, V] (the layout the reference's CPU path
     indexes for batch_first == false, cpu_rnnt.h:139-144); labels [N, U-1], lengths and costs [N].
-    fp32 / fp64, no host synchronisation.  Returns the workspace tensor.  Gradient and lattice options as
-    gpu_rnnt_async."""
+    fp32 / fp64, no host synchronisation.  Returns the workspace tensor.  Gradient and lattice options and the
+    topology as gpu_rnnt_async."""
     T, U, N, V = acts.shape
     return _loss_async(RNNT_B200_LAYOUT_TUNV, T, U, N, V, acts, labels, input_lengths, label_lengths, costs, grads,
-                       blank_label, grad_scale, workspace, fastemit_lambda, clamp, delay_penalty)
+                       blank_label, grad_scale, workspace, fastemit_lambda, clamp, delay_penalty, rnnt_type)
 
 
 def _code16(acts):
@@ -306,12 +335,13 @@ def costs_dtype(acts):
 
 
 def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_label,
-                     prepare_backward=True, workspace=None, *, delay_penalty=0.0):
+                     prepare_backward=True, workspace=None, *, delay_penalty=0.0, rnnt_type='regular'):
     """Training-step split, first half: statistics + lattices into `workspace`, costs on the
     device, no synchronisation.  Returns the workspace tensor (hand it to gpu_rnnt_backward, with the same
-    delay_penalty)."""
+    delay_penalty and rnnt_type)."""
     N, T, U, V = acts.shape
     lopt = lattice_options(delay_penalty)
+    topo = rnnt_type_code(rnnt_type)
     code = _code16(acts)
     fn = {torch.float32: _lib.rnnt_b200_forward, torch.float64: _lib.rnnt_b200_forward_fp64}.get(acts.dtype)
     if code is None and fn is None:
@@ -321,7 +351,9 @@ def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_la
         args = (acts.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(), input_lengths.data_ptr(),
                 V, N, costs.data_ptr(), 1 if prepare_backward else 0)
         tail = (workspace.data_ptr(), _options(acts, blank_label))
-        if lopt is not None:
+        if topo != RNNT_B200_RNNT_REGULAR:
+            st = _lib.rnnt_b200_forward_topo(_dtype_code(acts), *args, lopt or rnntLatticeOptions(), topo, *tail)
+        elif lopt is not None:
             st = _lib.rnnt_b200_forward_lat(_dtype_code(acts), *args, lopt, *tail)
         else:
             st = _lib.rnnt_b200_forward_16(code, *args, *tail) if code else fn(*args, *tail)
@@ -331,20 +363,24 @@ def gpu_rnnt_forward(acts, labels, input_lengths, label_lengths, costs, blank_la
 
 
 def gpu_rnnt_backward(acts, labels, input_lengths, label_lengths, grads, grad_costs, blank_label,
-                      grad_scale, workspace, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0):
+                      grad_scale, workspace, *, fastemit_lambda=0.0, clamp=-1.0, delay_penalty=0.0,
+                      rnnt_type='regular'):
     """Second half: grads[b] = grad_scale * grad_costs[b] * d cost[b] / d acts[b] from the lattices
     gpu_rnnt_forward left in `workspace` (grad_costs: device tensor [N] or None for ones).
     With gradient options (see grad_options): grad_scale * grad_costs[b] * clip(g[b]), g[b] the FastEmit
-    gradient when fastemit_lambda > 0.  delay_penalty: the one the forward half got."""
+    gradient when fastemit_lambda > 0.  delay_penalty and rnnt_type: the ones the forward half got."""
     N, T, U, V = acts.shape
     gopt = _ex_options(fastemit_lambda, clamp)
     lopt = lattice_options(delay_penalty)
+    topo = rnnt_type_code(rnnt_type)
     code = _dtype_code(acts)
     with torch.cuda.device(acts.device):
         args = (code, acts.data_ptr(), grads.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(),
                 input_lengths.data_ptr(), V, N, _ptr(grad_costs), grad_scale, gopt)
         tail = (workspace.data_ptr(), _options(acts, blank_label))
-        if lopt is None:
+        if topo != RNNT_B200_RNNT_REGULAR:
+            st = _lib.rnnt_b200_backward_topo(*args, lopt or rnntLatticeOptions(), topo, *tail)
+        elif lopt is None:
             st = _lib.rnnt_b200_backward_ex(*args, *tail)
         else:
             st = _lib.rnnt_b200_backward_lat(*args, lopt, *tail)
