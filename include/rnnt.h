@@ -569,6 +569,40 @@ rnntStatus_t rnnt_b200_add_joint_prune_ranges_topo(const int* label_lengths, con
                                                    int s_range, int* ranges, const void* workspace, int rnnt_type,
                                                    struct rnntOptions options);
 
+/* Forced alignment (DESIGN.md §12): the highest-scoring path through the lattice of each utterance, and the frame
+ * at which it emits each label.  The lattice is the loss's: T_b, U_b = label_length + 1 after the loss's clamps,
+ * and the natural-log blank / label log-probabilities lp_0(t,u), lp_y(t,u) of the dense (or pruned, uncovered cells
+ * at log zero) logits.  No delay penalty is applied.
+ *   RNNT_B200_RNNT_REGULAR   an alignment is one frame per label, t_0 <= t_1 <= ... <= t_{U_b-2} in [0, T_b-1]:
+ *                            label j is emitted from cell (t_j, j), the blank of frame t from (t, #{j : t_j <= t});
+ *                            T_b + U_b - 1 factors.
+ *   RNNT_B200_RNNT_MODIFIED  frames strictly increase, t_0 < t_1 < ...: frame t_j emits label j from (t_j, j), every
+ *                            other frame t a blank from (t, #{j : t_j < t}); T_b factors.
+ * Outputs, every element written:
+ *   frames [N, maxU-1] int32: t_j of the best alignment; -1 for j >= label_length.
+ *   scores [N]: that alignment's log-probability (natural log, <= 0; the sign is opposite to the costs), float for
+ *          RNNT_B200_FP32 / _BF16 / _FP16, double for RNNT_B200_FP64.
+ * Ties: where the two predecessors of a cell score exactly equal, the blank predecessor (t-1, u) wins, so among equal
+ * partial paths labels are emitted as early as possible (uniform logits: regular - every label at frame 0,
+ * modified - label j at frame j).
+ * No path (best score log zero: a modified utterance with U_b - 1 > T_b, windows without a path, -inf logits):
+ * scores[b] = -inf and frames[b, :] = -1.  A NaN factor: scores[b] = NaN and frames[b, :] = -1.  Other utterances
+ * are unaffected.
+ * dtype is RNNT_B200_FP32, _FP64, _BF16 or _FP16; layout NTUV or TUNV (TUNV: FP32 / FP64 only); the pruned entry
+ * takes [N, maxT, s_range, V] logits and `ranges` as rnnt_b200_pruned_loss_async_topo.  All pointers are device
+ * pointers; the call is stream-ordered on options.stream and does not synchronise.  The workspace is that of the
+ * loss: get_workspace_size / rnnt_b200_pruned_workspace_size.  Arguments the loss entries reject, an unknown dtype,
+ * layout or rnnt_type, s_range < 1 and NULL pointers (frames may be NULL when maxU == 1) are
+ * RNNT_STATUS_INVALID_VALUE before any device access. */
+rnntStatus_t rnnt_b200_align(int dtype, int layout, const void* activations, const int* flat_labels,
+                             const int* label_lengths, const int* input_lengths, int alphabet_size, int minibatch,
+                             int rnnt_type, int* frames, void* scores_device, void* workspace,
+                             struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_align(int dtype, const void* activations, const int* ranges, int s_range,
+                                    const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                    int alphabet_size, int minibatch, int rnnt_type, int* frames,
+                                    void* scores_device, void* workspace, struct rnntOptions options);
+
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug
  * builds (include/detail/cpu_rnnt.h:167-170); tests/test_gpu_round2.py does the same.  Synchronises. */

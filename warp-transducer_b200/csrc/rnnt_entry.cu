@@ -22,6 +22,7 @@
 #include "rnnt_joint.cuh"
 #include "rnnt_kernels.cuh"
 #include "rnnt_lattice.cuh"
+#include "rnnt_viterbi.cuh"
 
 using namespace b200rnnt;
 
@@ -293,8 +294,9 @@ template <typename T> GradReg<T> make_grad_reg(const rnntGradOptions& o, const W
 
 // What a call does.  The reference API is FULL (stats -> lattice -> grad in one call); the
 // operator splits a training step into FORWARD (stats + both lattices, costs out) and BACKWARD
-// (gradient pass only, reading the lattices the forward left in the workspace).
-enum Phase { kFull = 0, kForward = 1, kBackward = 2 };
+// (gradient pass only, reading the lattices the forward left in the workspace).  ALIGN is forced alignment
+// (DESIGN.md §12): pass 1, then the Viterbi wavefront and its backtrace; the costs are the best paths' scores.
+enum Phase { kFull = 0, kForward = 1, kBackward = 2, kAlign = 3 };
 
 // What one compute call asks for, besides its tensors.
 struct Call {
@@ -319,6 +321,11 @@ Call forward_call(int prepare_backward) {
 Call backward_call(double scale, const void* grad_costs, rnntGradOptions grad = {0.0f, 0.0f}) {
     return Call{kBackward, true, false, false, scale, grad_costs, grad};
 }
+Call align_call(bool tunv, int rnnt_type) {
+    Call c{kAlign, true, false, tunv, 1.0, nullptr, {0.0f, 0.0f}};
+    c.rnnt_type = rnnt_type;
+    return c;
+}
 
 // The tensors and extents of a call, in the order the C-ABI entries take them.  For the additive joint, acts
 // and grads are the transcription factor and its gradient.
@@ -332,6 +339,7 @@ struct Tensors {
     rnntOptions opt;
     const int* ranges = nullptr;   // pruned calls: [N, maxT] window starts
     int s_range = 0;               // pruned calls: R, rows per frame
+    int* frames = nullptr;         // alignment calls: [N, maxU-1] label frames (NULL allowed when maxU == 1)
 };
 
 // The checks of every compute call, all before any device access; the first that fails decides the status.
@@ -343,6 +351,7 @@ rnntStatus_t check_call(const Tensors& t, const Call& c) {
     if (!t.acts || !t.labels || !t.ylen || !t.xlen || (!t.costs && c.phase != kBackward) || !t.workspace ||
         t.V <= 0 || t.N <= 0 || opt.maxT <= 0 || opt.maxU <= 0 || (c.phase == kBackward && !t.grads))
         return RNNT_STATUS_INVALID_VALUE;  // reference src/rnnt_entrypoint.cpp:49-59
+    if (c.phase == kAlign && (t.grads || (!t.frames && opt.maxU > 1))) return RNNT_STATUS_INVALID_VALUE;
     // pruned rows are counted with 32 bits like the dense ones; the pruned kernels index [N,maxT,R,V] only
     if (c.pruned && (!t.ranges || t.s_range < 1 || c.tunv || (uint64_t)t.N * opt.maxT * t.s_range >= (1ull << 31)))
         return RNNT_STATUS_INVALID_VALUE;
@@ -679,6 +688,34 @@ void launch_lattice_lin(const float4* lp2, const int* xlen, const int* ylen, Log
     else launch(lattice_lin_kernel<1, true, 8>, kLinStaticSmem);
 }
 
+// Forced alignment (rnnt_viterbi.cuh): one CTA per utterance, one thread per label column, a kRing-deep factor ring.
+// The decision bits take the alphas section, which an alignment call does not otherwise use.
+template <typename T>
+void launch_viterbi(const void* lp2, const int* xlen, const int* ylen, void* alphas, int* frames, T* scores,
+                    const Dims& d, bool mod, cudaStream_t s) {
+    const int threads = viterbi_words(d.maxU) * 32;
+    const size_t ring = (size_t)kRing * threads * 16;
+    auto launch = [&](auto kernel, auto fac) {
+        if (ring > 40 * 1024)
+            func_attr_once(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring);
+        kernel<<<d.N, threads, ring, s>>>(static_cast<decltype(fac)>(lp2), xlen, ylen, static_cast<uint32_t*>(alphas),
+                                          frames, scores, d);
+    };
+    if constexpr (sizeof(T) == 4) {
+        const float4* f = nullptr;
+        if (mod && threads > 32) launch(viterbi_lin_mod_kernel<true>, f);
+        else if (mod) launch(viterbi_lin_mod_kernel<false>, f);
+        else if (threads > 32) launch(viterbi_lin_kernel<true>, f);
+        else launch(viterbi_lin_kernel<false>, f);
+    } else {
+        const double2* f = nullptr;
+        if (mod && threads > 32) launch(viterbi_mod_kernel<true>, f);
+        else if (mod) launch(viterbi_mod_kernel<false>, f);
+        else if (threads > 32) launch(viterbi_kernel<true>, f);
+        else launch(viterbi_kernel<false>, f);
+    }
+}
+
 template <typename IO>
 rnntStatus_t run(const Tensors& t, const Call& c) {
     using T = typename ComputeOf<IO>::type;  // arithmetic type (float for the 16-bit storage types)
@@ -836,8 +873,14 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
             // pass 1: log-softmax statistics + (blank, label) log-prob gather
             stream_pass(g, 1);
             mark(1, s);
-            // lattice: alpha (and beta when gradients are or will be wanted)
-            launch_lattice(g, s);
+            if (c.phase == kAlign) {
+                // best path and its label frames (DESIGN.md §12)
+                launch_viterbi<T>(g.w.lp2, g.xlen, g.ylen, g.w.alphas, t.frames, g.costs, g.d, g.mod, s);
+                ++g_last_launches;
+            } else {
+                // lattice: alpha (and beta when gradients are or will be wanted)
+                launch_lattice(g, s);
+            }
         } else {
             mark(1, s);
         }
@@ -1733,6 +1776,29 @@ rnntStatus_t rnnt_b200_add_joint_prune_ranges(const int* label_lengths, const in
                                               int s_range, int* ranges, const void* workspace, rnntOptions options) {
     return rnnt_b200_add_joint_prune_ranges_topo(label_lengths, input_lengths, minibatch, s_range, ranges, workspace,
                                                  RNNT_B200_RNNT_REGULAR, options);
+}
+
+// ---- forced alignment (DESIGN.md §12): the best path's label frames and score, on the device ---------------
+rnntStatus_t rnnt_b200_align(int dtype, int layout, const void* activations, const int* flat_labels,
+                             const int* label_lengths, const int* input_lengths, int alphabet_size, int minibatch,
+                             int rnnt_type, int* frames, void* scores_device, void* workspace, rnntOptions options) {
+    const bool tunv = layout == RNNT_B200_LAYOUT_TUNV;
+    if (!is_layout(layout) || (tunv && is_16bit(dtype))) return RNNT_STATUS_INVALID_VALUE;
+    Tensors t{activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+              scores_device, workspace, options};
+    t.frames = frames;
+    return run_as(dtype, t, align_call(tunv, rnnt_type));
+}
+rnntStatus_t rnnt_b200_pruned_align(int dtype, const void* activations, const int* ranges, int s_range,
+                                    const int* flat_labels, const int* label_lengths, const int* input_lengths,
+                                    int alphabet_size, int minibatch, int rnnt_type, int* frames,
+                                    void* scores_device, void* workspace, rnntOptions options) {
+    Call c = align_call(false, rnnt_type);
+    c.pruned = true;
+    Tensors t{activations, nullptr, flat_labels, label_lengths, input_lengths, alphabet_size, minibatch,
+              scores_device, workspace, options, ranges, s_range};
+    t.frames = frames;
+    return run_as(dtype, t, c);
 }
 
 rnntStatus_t get_workspace_size(int maxT, int maxU, int minibatch, bool gpu, size_t* size_bytes,

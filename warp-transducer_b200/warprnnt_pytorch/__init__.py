@@ -6,7 +6,8 @@ blank=0, reduction='mean')`` and the ``warp_rnnt`` extension functions, with the
 input rules and error types (certify_inputs, :115-140).  Keyword-only additions:
 ``fastemit_lambda`` (FastEmit regularisation), ``clamp`` (element-wise gradient clipping),
 ``delay_penalty`` (the delay-penalised lattice of low-latency streaming training) and ``rnnt_type``
-(k2's 'regular' or 'modified' one-symbol-per-frame topology); see rnnt_loss.  Differences, all on the fast side:
+(k2's 'regular' or 'modified' one-symbol-per-frame topology); see rnnt_loss.  ``rnnt_forced_align`` and
+``pruned_rnnt_forced_align`` give the best path's label frames and score (forced alignment).  Differences, all on the fast side:
 the call never synchronises with the host except for the reference's own length check, costs
 stay on the device, and the gradient is produced in autograd's backward with grad_output and the
 'mean' factor folded into the kernel - no zeros_like / mul_ passes over the [N,T,U,V] tensor.
@@ -136,3 +137,6 @@ from .pruned import (PrunedRNNTLoss, add_joint_rnnt_loss_with_ranges, prune_join
                      pruned_rnnt_loss)
 
 __all__ += ['pruned_rnnt_loss', 'PrunedRNNTLoss', 'add_joint_rnnt_loss_with_ranges', 'prune_joint_inputs']
+from .align import pruned_rnnt_forced_align, rnnt_forced_align  # noqa: E402
+
+__all__ += ['rnnt_forced_align', 'pruned_rnnt_forced_align']

@@ -99,6 +99,11 @@ _lib.rnnt_b200_forward_topo.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_in
 _lib.rnnt_b200_backward_topo.restype = C.c_int
 _lib.rnnt_b200_backward_topo.argtypes = [C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double,
                                          rnntGradOptions, rnntLatticeOptions, C.c_int, _P, rnntOptions]
+_lib.rnnt_b200_align.restype = C.c_int
+_lib.rnnt_b200_align.argtypes = [C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, rnntOptions]
+_lib.rnnt_b200_pruned_align.restype = C.c_int
+_lib.rnnt_b200_pruned_align.argtypes = [C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P,
+                                        rnntOptions]
 _lib.get_workspace_size.restype = C.c_int
 _lib.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
 _lib.get_warprnnt_version.restype = C.c_int
@@ -387,6 +392,56 @@ def gpu_rnnt_backward(acts, labels, input_lengths, label_lengths, grads, grad_co
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_backward_ex failed: " + status_string(st))
     return 0
+
+
+def gpu_rnnt_align(acts, labels, input_lengths, label_lengths, frames, scores, blank_label, workspace=None, *,
+                   rnnt_type='regular', time_major=False):
+    """Forced alignment (include/rnnt.h rnnt_b200_align): the best path of each utterance's lattice.  Writes
+    frames [N, U-1] int32 (the frame of each label, -1 past label_lengths and without a path) and scores [N]
+    (its natural-log probability; costs_dtype(acts)), on the device, without synchronising.  acts: [N, T, U, V], or
+    [T, U, N, V] with time_major (fp32 / fp64).  Returns the workspace tensor."""
+    topo = rnnt_type_code(rnnt_type)
+    code = _dtype_code(acts)
+    layout = RNNT_B200_LAYOUT_TUNV if time_major else RNNT_B200_LAYOUT_NTUV
+    if time_major:
+        T, U, N, V = acts.shape
+        if code not in (RNNT_B200_FP32, RNNT_B200_FP64):
+            raise TypeError("unsupported data type %s for the time-major layout" % acts.dtype)
+    else:
+        N, T, U, V = acts.shape
+    with torch.cuda.device(acts.device):
+        workspace = _workspace(acts, T, U, N, workspace)
+        opt = _options(acts, blank_label)
+        opt.maxT, opt.maxU = T, U
+        st = _lib.rnnt_b200_align(code, layout, acts.data_ptr(), _labels_ptr(labels), label_lengths.data_ptr(),
+                                  input_lengths.data_ptr(), V, N, topo, _ptr(frames), scores.data_ptr(),
+                                  workspace.data_ptr(), opt)
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_align failed: " + status_string(st))
+    return workspace
+
+
+def gpu_pruned_rnnt_align(logits, ranges, labels, input_lengths, label_lengths, frames, scores, blank_label,
+                          workspace=None, *, rnnt_type='regular'):
+    """gpu_rnnt_align for pruned logits [N, T, R, V] over the windows `ranges` [N, T] (include/rnnt.h
+    rnnt_b200_pruned_align); the lattice is [T, labels.shape[1] + 1].  Returns the workspace tensor."""
+    from .pruned import pruned_workspace_size
+    topo = rnnt_type_code(rnnt_type)
+    code = _dtype_code(logits)
+    N, T, R, V = logits.shape
+    U = labels.shape[1] + 1
+    with torch.cuda.device(logits.device):
+        need = pruned_workspace_size(T, U, R, N, 8 if logits.dtype == torch.float64 else 4)
+        if workspace is None or workspace.numel() < need:
+            workspace = torch.empty(need, dtype=torch.uint8, device=logits.device)
+        opt = _options(logits, blank_label)
+        opt.maxT, opt.maxU = T, U
+        st = _lib.rnnt_b200_pruned_align(code, logits.data_ptr(), ranges.data_ptr(), R, _labels_ptr(labels),
+                                         label_lengths.data_ptr(), input_lengths.data_ptr(), V, N, topo,
+                                         _ptr(frames), scores.data_ptr(), workspace.data_ptr(), opt)
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_pruned_align failed: " + status_string(st))
+    return workspace
 
 
 _lib.rnnt_b200_debug_log_likelihoods.restype = C.c_int
