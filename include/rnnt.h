@@ -603,6 +603,43 @@ rnntStatus_t rnnt_b200_pruned_align(int dtype, const void* activations, const in
                                     int alphabet_size, int minibatch, int rnnt_type, int* frames,
                                     void* scores_device, void* workspace, struct rnntOptions options);
 
+/* The loss, its gradient and forced alignment on caller-supplied factors (DESIGN.md §13; k2's
+ * mutual_information_recursion).  The lattice machinery above without the log-softmax: the caller forms the
+ * natural-log transition factors, by any joiner, prior, fusion or penalty.  Inputs, label-major with t contiguous:
+ *   px [N, S, T]    px[b, s, t] = lp_y(t, s), the label factor out of cell (t, s) (emitting label s at frame t)
+ *   py [N, S+1, T]  py[b, s, t] = lp_0(t, s), the blank factor out of cell (t, s)
+ * with T = options.maxT and S + 1 = options.maxU; label_lengths / input_lengths give S_b and T_b (clamped as the loss
+ * clamps them: U_b = S_b + 1).  There are no labels, no blank index and no alphabet; options.blank_label is ignored.
+ * Factors need not be normalised: any finite value or -inf is valid, and positive factors give negative costs.  The
+ * fp32 arithmetic (RNNT_B200_FP32 / _BF16 / _FP16) represents factors of magnitude below 2^22 ln 2 (about 2.9e6).
+ *   RNNT_B200_RNNT_REGULAR   k2's -mutual_information_recursion(px with a -inf column T appended, py,
+ *                            boundary = [0, 0, S_b, T_b]): the recursion of the dense loss.
+ *   RNNT_B200_RNNT_MODIFIED  the same with k2's px of width T: one transition per frame (DESIGN.md §11).
+ * forward: costs[b] = -log-likelihood (float, double for RNNT_B200_FP64); +inf without a path; NaN when a factor of
+ *   the utterance is NaN or +inf.  prepare_backward: also the beta lattice, for a backward on the same workspace.
+ * backward: py_grad[b,s,t] = -g[b] e_0(t,s) and px_grad[b,s,t] = -g[b] e_y(t,s), the blank and label transition
+ *   occupancies (the exact gradient of the cost), g[b] = grad_scale * grad_costs_device[b] (arithmetic type; NULL:
+ *   ones); zero on padding (t >= T_b, s > S_b for py, s >= S_b for px) and for an utterance without a path.  It reads
+ *   only the workspace of a forward with prepare_backward and must get that forward's rnnt_type.
+ * align: frames [N, S] and scores [N] as rnnt_b200_align, on these factors.
+ * Other utterances' results do not depend on a NaN, +inf or -inf factor of one utterance.  dtype: RNNT_B200_FP32,
+ * _FP64, _BF16 or _FP16, for px, py and the gradients alike.  All pointers are device pointers; the calls are
+ * stream-ordered on options.stream and do not synchronise.  The workspace is rnnt_b200_lattice_workspace_size's.  An
+ * unknown dtype or rnnt_type, NULL pointers (px, px_grad and frames may be NULL when maxU == 1), minibatch, maxT or
+ * maxU < 1, maxU > 1024 and minibatch * maxT * maxU >= 2^31 are RNNT_STATUS_INVALID_VALUE before any device access. */
+rnntStatus_t rnnt_b200_lattice_workspace_size(int maxT, int maxU, int minibatch, size_t dtype_size,
+                                              size_t* size_bytes);
+rnntStatus_t rnnt_b200_lattice_forward(int dtype, const void* px, const void* py, const int* label_lengths,
+                                       const int* input_lengths, int minibatch, int rnnt_type, void* costs_device,
+                                       int prepare_backward, void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_lattice_backward(int dtype, void* px_grad, void* py_grad, const int* label_lengths,
+                                        const int* input_lengths, int minibatch, int rnnt_type,
+                                        const void* grad_costs_device, double grad_scale, void* workspace,
+                                        struct rnntOptions options);
+rnntStatus_t rnnt_b200_lattice_align(int dtype, const void* px, const void* py, const int* label_lengths,
+                                     const int* input_lengths, int minibatch, int rnnt_type, int* frames,
+                                     void* scores_device, void* workspace, struct rnntOptions options);
+
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug
  * builds (include/detail/cpu_rnnt.h:167-170); tests/test_gpu_round2.py does the same.  Synchronises. */

@@ -22,6 +22,7 @@
 #include "rnnt_joint.cuh"
 #include "rnnt_kernels.cuh"
 #include "rnnt_lattice.cuh"
+#include "rnnt_lattice_io.cuh"
 #include "rnnt_viterbi.cuh"
 
 using namespace b200rnnt;
@@ -688,6 +689,27 @@ void launch_lattice_lin(const float4* lp2, const int* xlen, const int* ylen, Log
     else launch(lattice_lin_kernel<1, true, 8>, kLinStaticSmem);
 }
 
+// fp64 lattice: log-domain wavefront (rnnt_kernels.cuh), one thread per label column; alpha, and beta in a second
+// grid row when with_beta.  mod: the modified topology (DESIGN.md §11).
+void launch_lattice_log(const double2* lp2, const int* xlen, const int* ylen, double* alphas, double* betas,
+                        double* llf, double* llb, double* costs, const Dims& d, bool with_beta, cudaStream_t s,
+                        bool pdl, bool mod) {
+    const int threads = (d.maxU + 31) / 32 * 32;
+    const size_t ring = (size_t)kRing * threads * sizeof(double2);
+    auto launch = [&](auto kernel) {
+        // opt-in when static + dynamic shared memory exceed the 48 KB default (maxU >= 353);
+        // the attribute is per device and the call is rare and cheap next to such a wavefront
+        if (ring + kLatticeStaticSmem > 48 * 1024)
+            cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring);
+        launch_k(kernel, dim3(d.N, with_beta ? 2 : 1), dim3(threads), ring, s, pdl, lp2, xlen, ylen, alphas, betas,
+                 llf, llb, costs, d);
+    };
+    if (mod && threads > 32) launch(lattice_mod_kernel<double, true>);
+    else if (mod) launch(lattice_mod_kernel<double, false>);
+    else if (threads > 32) launch(lattice_kernel<double, true>);
+    else launch(lattice_kernel<double, false>);
+}
+
 // Forced alignment (rnnt_viterbi.cuh): one CTA per utterance, one thread per label column, a kRing-deep factor ring.
 // The decision bits take the alphas section, which an alignment call does not otherwise use.
 template <typename T>
@@ -837,23 +859,9 @@ rnntStatus_t run(const Tensors& t, const Call& c) {
                                static_cast<LogVal*>(g.w.llb), g.costs, g.d, with_beta,
                                lattice_ring_depth(opt.maxU, co_running, hooks().lat_ring), st, g.pdl, g.mod);
         } else {
-            // fp64: log-domain wavefront (rnnt_kernels.cuh)
-            const int threads = (opt.maxU + 31) / 32 * 32;
-            const size_t ring = (size_t)kRing * threads * sizeof(double2);
-            auto launch = [&](auto kernel) {
-                // opt-in when static + dynamic shared memory exceed the 48 KB default (maxU >= 353);
-                // the attribute is per device and the call is rare and cheap next to such a wavefront
-                if (ring + kLatticeStaticSmem > 48 * 1024)
-                    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ring);
-                launch_k(kernel, dim3(g.d.N, with_beta ? 2 : 1), dim3(threads), ring, st, g.pdl,
-                         static_cast<const double2*>(g.w.lp2), g.xlen, g.ylen, static_cast<double*>(g.w.alphas),
-                         static_cast<double*>(g.w.betas), static_cast<double*>(g.w.llf),
-                         static_cast<double*>(g.w.llb), g.costs, g.d);
-            };
-            if (g.mod && threads > 32) launch(lattice_mod_kernel<double, true>);
-            else if (g.mod) launch(lattice_mod_kernel<double, false>);
-            else if (threads > 32) launch(lattice_kernel<double, true>);
-            else launch(lattice_kernel<double, false>);
+            launch_lattice_log(static_cast<const double2*>(g.w.lp2), g.xlen, g.ylen, static_cast<double*>(g.w.alphas),
+                               static_cast<double*>(g.w.betas), static_cast<double*>(g.w.llf),
+                               static_cast<double*>(g.w.llb), g.costs, g.d, with_beta, st, g.pdl, g.mod);
         }
         ++g_last_launches;
     };
@@ -1281,6 +1289,101 @@ rnntStatus_t run_as(int dtype, const Tensors& t, const Call& c) {
 }
 inline bool is_16bit(int dtype) { return dtype == RNNT_B200_BF16 || dtype == RNNT_B200_FP16; }
 inline bool is_layout(int layout) { return layout == RNNT_B200_LAYOUT_NTUV || layout == RNNT_B200_LAYOUT_TUNV; }
+
+// ---- the loss, gradient and alignment on caller-supplied factors (DESIGN.md §13) --------------------------------
+// The tensors of a lattice call: px [N, maxU-1, maxT], py [N, maxU, maxT] and their gradients in the storage type.
+struct LatticeTensors {
+    const void *px, *py;
+    void *px_grad, *py_grad;   // backward
+    const int *ylen, *xlen;
+    int N;
+    void* costs;               // forward: costs; align: scores (arithmetic type)
+    int* frames;               // align
+    void* workspace;
+    rnntOptions opt;
+};
+
+inline size_t lattice_cells(int N, int maxT, int maxU) { return (size_t)N * (maxT + maxU - 1) * maxU; }
+
+// check_call's extent rules without its V and blank rules; every check before any device access.  px, px_grad and
+// frames have no element when maxU == 1 and may then be NULL.
+rnntStatus_t check_lattice(int dtype, const LatticeTensors& t, const Call& c) {
+    const rnntOptions& opt = t.opt;
+    if ((dtype != RNNT_B200_FP32 && dtype != RNNT_B200_FP64 && !is_16bit(dtype)) ||
+        (c.rnnt_type != RNNT_B200_RNNT_REGULAR && c.rnnt_type != RNNT_B200_RNNT_MODIFIED))
+        return RNNT_STATUS_INVALID_VALUE;
+    const bool labels = opt.maxU > 1;
+    if (!t.ylen || !t.xlen || !t.workspace || t.N <= 0 || opt.maxT <= 0 || opt.maxU <= 0)
+        return RNNT_STATUS_INVALID_VALUE;
+    if (c.phase == kBackward ? (!t.py_grad || (labels && !t.px_grad))
+                             : (!t.py || (labels && !t.px) || !t.costs || (c.phase == kAlign && labels && !t.frames)))
+        return RNNT_STATUS_INVALID_VALUE;
+    if (opt.loc == RNNT_CPU) {
+        fprintf(stderr, "b200-rnnt: CPU execution requested, but this library is the CUDA path only\n");
+        return RNNT_STATUS_EXECUTION_FAILED;
+    }
+    if (opt.loc != RNNT_GPU || (uint64_t)t.N * opt.maxT * opt.maxU >= (1ull << 31) || opt.maxU > 1024)
+        return RNNT_STATUS_INVALID_VALUE;
+    return RNNT_STATUS_SUCCESS;
+}
+
+// One batch group, no PDL, no host synchronisation.  Forward: import, then the wavefront (alpha, and beta when
+// want_beta) - 2 launches.  Backward: the gradient kernel on the workspace alone - 1.  Align: import, then the
+// Viterbi kernel - 2.
+template <typename IO>
+rnntStatus_t run_lattice(const LatticeTensors& t, const Call& c) {
+    using T = typename ComputeOf<IO>::type;
+    const rnntOptions& opt = t.opt;
+    const int N = t.N;
+    g_last_launches = 0;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(opt.stream);
+    Workspace w = carve(t.workspace, 0, lattice_cells(N, opt.maxT, opt.maxU), N, opt.maxU, sizeof(T));
+    Tensors dt{nullptr, nullptr, nullptr, t.ylen, t.xlen, 1, N, nullptr, nullptr, opt};
+    dt.opt.blank_label = 0;
+    const Dims d = make_dims(dt, false);
+    const bool mod = c.rnnt_type == RNNT_B200_RNNT_MODIFIED;
+    using Fac = typename Lat<T>::fac;
+    using Val = typename Lat<T>::val;
+    const unsigned blocks = lattice_io_blocks(d);
+    T* costs = static_cast<T*>(t.costs);
+    if (c.phase != kBackward) {
+        lattice_import_kernel<IO><<<blocks, 256, 0, s>>>(static_cast<const IO*>(t.px), static_cast<const IO*>(t.py),
+                                                        t.xlen, t.ylen, static_cast<Fac*>(w.lp2), d);
+        ++g_last_launches;
+    }
+    if (c.phase == kForward) {
+        if constexpr (sizeof(T) == 4)
+            launch_lattice_lin(static_cast<const float4*>(w.lp2), t.xlen, t.ylen, static_cast<LogVal*>(w.alphas),
+                               static_cast<LogVal*>(w.betas), static_cast<LogVal*>(w.llf),
+                               static_cast<LogVal*>(w.llb), costs, d, c.want_beta,
+                               lattice_ring_depth(opt.maxU, false, hooks().lat_ring), s, false, mod);
+        else
+            launch_lattice_log(static_cast<const double2*>(w.lp2), t.xlen, t.ylen, static_cast<double*>(w.alphas),
+                               static_cast<double*>(w.betas), static_cast<double*>(w.llf),
+                               static_cast<double*>(w.llb), costs, d, c.want_beta, s, false, mod);
+    } else if (c.phase == kAlign) {
+        launch_viterbi<T>(w.lp2, t.xlen, t.ylen, w.alphas, t.frames, costs, d, mod, s);
+    } else {
+        auto kernel = mod ? lattice_grad_kernel<IO, T, true> : lattice_grad_kernel<IO, T, false>;
+        kernel<<<blocks, 256, 0, s>>>(static_cast<const Fac*>(w.lp2), static_cast<const Val*>(w.alphas),
+                                      static_cast<const Val*>(w.betas), static_cast<const Val*>(w.llf), t.xlen, t.ylen,
+                                      static_cast<IO*>(t.px_grad), static_cast<IO*>(t.py_grad), (T)c.scale,
+                                      static_cast<const T*>(c.scale_vec), d);
+    }
+    ++g_last_launches;
+    return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED;
+}
+
+rnntStatus_t run_lattice_as(int dtype, const LatticeTensors& t, const Call& c) {
+    if (const rnntStatus_t st = check_lattice(dtype, t, c)) return st;
+    switch (dtype) {
+        case RNNT_B200_FP32: return run_lattice<float>(t, c);
+        case RNNT_B200_FP64: return run_lattice<double>(t, c);
+        case RNNT_B200_BF16: return run_lattice<__nv_bfloat16>(t, c);
+        case RNNT_B200_FP16: return run_lattice<__half>(t, c);
+    }
+    return RNNT_STATUS_INVALID_VALUE;
+}
 
 }  // namespace
 
@@ -1799,6 +1902,41 @@ rnntStatus_t rnnt_b200_pruned_align(int dtype, const void* activations, const in
               scores_device, workspace, options, ranges, s_range};
     t.frames = frames;
     return run_as(dtype, t, c);
+}
+
+// ---- the loss, gradient and alignment on caller-supplied factors (DESIGN.md §13) -------------------------------
+rnntStatus_t rnnt_b200_lattice_workspace_size(int maxT, int maxU, int minibatch, size_t dtype_size,
+                                              size_t* size_bytes) {
+    if (minibatch <= 0 || maxT <= 0 || maxU <= 0 || size_bytes == nullptr) return RNNT_STATUS_INVALID_VALUE;
+    if (dtype_size != sizeof(double)) dtype_size = sizeof(float);
+    *size_bytes = carve(nullptr, 0, lattice_cells(minibatch, maxT, maxU), minibatch, maxU, dtype_size).bytes;
+    return RNNT_STATUS_SUCCESS;
+}
+
+rnntStatus_t rnnt_b200_lattice_forward(int dtype, const void* px, const void* py, const int* label_lengths,
+                                       const int* input_lengths, int minibatch, int rnnt_type, void* costs_device,
+                                       int prepare_backward, void* workspace, rnntOptions options) {
+    Call c = forward_call(prepare_backward);
+    c.rnnt_type = rnnt_type;
+    return run_lattice_as(dtype, {px, py, nullptr, nullptr, label_lengths, input_lengths, minibatch, costs_device,
+                                  nullptr, workspace, options}, c);
+}
+
+rnntStatus_t rnnt_b200_lattice_backward(int dtype, void* px_grad, void* py_grad, const int* label_lengths,
+                                        const int* input_lengths, int minibatch, int rnnt_type,
+                                        const void* grad_costs_device, double grad_scale, void* workspace,
+                                        rnntOptions options) {
+    Call c = backward_call(grad_scale, grad_costs_device);
+    c.rnnt_type = rnnt_type;
+    return run_lattice_as(dtype, {nullptr, nullptr, px_grad, py_grad, label_lengths, input_lengths, minibatch, nullptr,
+                                  nullptr, workspace, options}, c);
+}
+
+rnntStatus_t rnnt_b200_lattice_align(int dtype, const void* px, const void* py, const int* label_lengths,
+                                     const int* input_lengths, int minibatch, int rnnt_type, int* frames,
+                                     void* scores_device, void* workspace, rnntOptions options) {
+    return run_lattice_as(dtype, {px, py, nullptr, nullptr, label_lengths, input_lengths, minibatch, scores_device,
+                                  frames, workspace, options}, align_call(false, rnnt_type));
 }
 
 rnntStatus_t get_workspace_size(int maxT, int maxU, int minibatch, bool gpu, size_t* size_bytes,

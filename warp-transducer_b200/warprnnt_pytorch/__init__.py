@@ -7,7 +7,9 @@ input rules and error types (certify_inputs, :115-140).  Keyword-only additions:
 ``fastemit_lambda`` (FastEmit regularisation), ``clamp`` (element-wise gradient clipping),
 ``delay_penalty`` (the delay-penalised lattice of low-latency streaming training) and ``rnnt_type``
 (k2's 'regular' or 'modified' one-symbol-per-frame topology); see rnnt_loss.  ``rnnt_forced_align`` and
-``pruned_rnnt_forced_align`` give the best path's label frames and score (forced alignment).  Differences, all on the fast side:
+``pruned_rnnt_forced_align`` give the best path's label frames and score (forced alignment).  ``rnnt_lattice_loss``,
+``RNNTLatticeLoss`` and ``rnnt_lattice_forced_align`` run the loss, gradient and alignment on blank and label
+log-probabilities the caller formed (k2's mutual_information_recursion).  Differences, all on the fast side:
 the call never synchronises with the host except for the reference's own length check, costs
 stay on the device, and the gradient is produced in autograd's backward with grad_output and the
 'mean' factor folded into the kernel - no zeros_like / mul_ passes over the [N,T,U,V] tensor.
@@ -140,3 +142,6 @@ __all__ += ['pruned_rnnt_loss', 'PrunedRNNTLoss', 'add_joint_rnnt_loss_with_rang
 from .align import pruned_rnnt_forced_align, rnnt_forced_align  # noqa: E402
 
 __all__ += ['rnnt_forced_align', 'pruned_rnnt_forced_align']
+from .lattice import RNNTLatticeLoss, rnnt_lattice_forced_align, rnnt_lattice_loss  # noqa: E402
+
+__all__ += ['rnnt_lattice_loss', 'RNNTLatticeLoss', 'rnnt_lattice_forced_align']

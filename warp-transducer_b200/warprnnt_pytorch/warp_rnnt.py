@@ -104,6 +104,15 @@ _lib.rnnt_b200_align.argtypes = [C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_
 _lib.rnnt_b200_pruned_align.restype = C.c_int
 _lib.rnnt_b200_pruned_align.argtypes = [C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P,
                                         rnntOptions]
+_lib.rnnt_b200_lattice_workspace_size.restype = C.c_int
+_lib.rnnt_b200_lattice_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)]
+_lib.rnnt_b200_lattice_forward.restype = C.c_int
+_lib.rnnt_b200_lattice_forward.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int, _P, rnntOptions]
+_lib.rnnt_b200_lattice_backward.restype = C.c_int
+_lib.rnnt_b200_lattice_backward.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_double, _P,
+                                            rnntOptions]
+_lib.rnnt_b200_lattice_align.restype = C.c_int
+_lib.rnnt_b200_lattice_align.argtypes = [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, rnntOptions]
 _lib.get_workspace_size.restype = C.c_int
 _lib.get_workspace_size.argtypes = [C.c_int, C.c_int, C.c_int, C.c_bool, C.POINTER(C.c_size_t), C.c_size_t]
 _lib.get_warprnnt_version.restype = C.c_int
@@ -441,6 +450,82 @@ def gpu_pruned_rnnt_align(logits, ranges, labels, input_lengths, label_lengths, 
                                          _ptr(frames), scores.data_ptr(), workspace.data_ptr(), opt)
     if st != RNNT_STATUS_SUCCESS:
         raise RuntimeError("rnnt_b200_pruned_align failed: " + status_string(st))
+    return workspace
+
+
+def lattice_workspace_size(maxT, maxU, minibatch, dtype_size=4):
+    """Bytes of workspace the lattice entries (include/rnnt.h rnnt_b200_lattice_forward) need."""
+    n = C.c_size_t(0)
+    st = _lib.rnnt_b200_lattice_workspace_size(maxT, maxU, minibatch, dtype_size, C.byref(n))
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_lattice_workspace_size failed: " + status_string(st))
+    return n.value
+
+
+def _lattice_options(py):
+    """rnntOptions of a lattice call: extents from py [N, S+1, T], the current stream of py's device."""
+    opt = rnntOptions()
+    opt.loc = RNNT_GPU
+    opt.stream = torch.cuda.current_stream(py.device).cuda_stream
+    opt.maxU, opt.maxT = py.size(1), py.size(2)
+    opt.batch_first = True
+    return opt
+
+
+def gpu_lattice_forward(px, py, input_lengths, label_lengths, costs, prepare_backward=True, workspace=None, *,
+                        rnnt_type='regular'):
+    """Loss on caller-supplied factors (include/rnnt.h rnnt_b200_lattice_forward): px [N, S, T] label and
+    py [N, S+1, T] blank log-factors, contiguous, one storage type.  Writes costs [N] (costs_dtype(py)) on the device
+    without synchronising; with prepare_backward the workspace also holds what gpu_lattice_backward reads.  Returns
+    the workspace tensor."""
+    topo = rnnt_type_code(rnnt_type)
+    code = _dtype_code(py)
+    N, U, T = py.shape
+    with torch.cuda.device(py.device):
+        need = lattice_workspace_size(T, U, N, 8 if py.dtype == torch.float64 else 4)
+        if workspace is None or workspace.numel() < need:
+            workspace = torch.empty(need, dtype=torch.uint8, device=py.device)
+        st = _lib.rnnt_b200_lattice_forward(code, _ptr(px), py.data_ptr(), label_lengths.data_ptr(),
+                                            input_lengths.data_ptr(), N, topo, costs.data_ptr(),
+                                            1 if prepare_backward else 0, workspace.data_ptr(), _lattice_options(py))
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_lattice_forward failed: " + status_string(st))
+    return workspace
+
+
+def gpu_lattice_backward(px_grad, py_grad, input_lengths, label_lengths, grad_costs, grad_scale, workspace, *,
+                         rnnt_type='regular'):
+    """Second half: px_grad / py_grad (shaped and typed as px / py) = grad_scale * grad_costs[b] * d cost[b] / d
+    px / py from the workspace gpu_lattice_forward(prepare_backward=True) filled, with the same rnnt_type.
+    grad_costs: device tensor [N] in costs_dtype, or None for ones.  Every element is written."""
+    topo = rnnt_type_code(rnnt_type)
+    code = _dtype_code(py_grad)
+    N = py_grad.size(0)
+    with torch.cuda.device(py_grad.device):
+        st = _lib.rnnt_b200_lattice_backward(code, _ptr(px_grad), py_grad.data_ptr(), label_lengths.data_ptr(),
+                                             input_lengths.data_ptr(), N, topo, _ptr(grad_costs), grad_scale,
+                                             workspace.data_ptr(), _lattice_options(py_grad))
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_lattice_backward failed: " + status_string(st))
+    return 0
+
+
+def gpu_lattice_align(px, py, input_lengths, label_lengths, frames, scores, workspace=None, *, rnnt_type='regular'):
+    """Forced alignment on caller-supplied factors (include/rnnt.h rnnt_b200_lattice_align): frames [N, S] int32
+    and scores [N] (costs_dtype(py)) as gpu_rnnt_align, on the device, without synchronising.  Returns the
+    workspace tensor."""
+    topo = rnnt_type_code(rnnt_type)
+    code = _dtype_code(py)
+    N, U, T = py.shape
+    with torch.cuda.device(py.device):
+        need = lattice_workspace_size(T, U, N, 8 if py.dtype == torch.float64 else 4)
+        if workspace is None or workspace.numel() < need:
+            workspace = torch.empty(need, dtype=torch.uint8, device=py.device)
+        st = _lib.rnnt_b200_lattice_align(code, _ptr(px), py.data_ptr(), label_lengths.data_ptr(),
+                                          input_lengths.data_ptr(), N, topo, _ptr(frames), scores.data_ptr(),
+                                          workspace.data_ptr(), _lattice_options(py))
+    if st != RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_lattice_align failed: " + status_string(st))
     return workspace
 
 
