@@ -640,6 +640,55 @@ rnntStatus_t rnnt_b200_lattice_align(int dtype, const void* px, const void* py, 
                                      const int* input_lengths, int minibatch, int rnnt_type, int* frames,
                                      void* scores_device, void* workspace, struct rnntOptions options);
 
+/* Fused joiner (DESIGN.md §14): the lattice factors of icefall's / torchaudio's / NeMo's joiner
+ *   logits[b,t,u,:] = weight act(enc[b,t] + pred[b,u]) + bias
+ * without forming the [N, T, U, V] logits, and the gradients of the four inputs back from the factors' gradients.
+ * Inputs, all bf16 device pointers, row-major and 16-byte aligned (bias: 2-byte):
+ *   enc [N, maxT, hidden], pred [N, maxU, hidden], weight [alphabet_size, hidden] (nn.Linear's layout),
+ *   bias [alphabet_size] or NULL (zero).
+ * flat_labels [N, maxU-1], label_lengths and input_lengths are int32 device pointers, as the loss takes them (S_b and
+ * T_b clamped into [0, maxU-1] and [1, maxT], as the lattice clamps them); options.blank_label is the blank column.
+ * forward: with h = round_bf16(act(fp32(enc[b,t]) + fp32(pred[b,u]))) (act: tanhf or relu), logit_v = sum_k h_k
+ *   weight[v,k] in fp32 plus fp32(bias[v]) and lse the fp32 logsumexp over all alphabet_size columns,
+ *   py [N, maxU, maxT]    py[b,u,t] = logit_blank - lse
+ *   px [N, maxU-1, maxT]  px[b,u,t] = logit_{labels[b,u]} - lse          (float; rnnt_b200_lattice_forward's layout)
+ *   -inf on padding (t >= T_b; u > S_b for py, u >= S_b for px).  Labels are compared with column indices, never used
+ *   as addresses: a label outside [0, alphabet_size) gives px = NaN on its row.  Padded rows of enc and pred are not
+ *   read.  The workspace keeps one fp32 lse per cell for the backward.
+ * backward: from dpx, dpy (float, the factors' gradients) and the workspace of a forward with the same arguments,
+ *   dlogit_v = dpy [v = blank] + dpx [v = label] - (dpx + dpy) softmax_v, rounded to bf16 in a chunk scratch;
+ *   grad_weight = sum dlogit (x) h, grad_bias = sum dlogit, ds = (dlogit weight) act'(s) (tanh: 1 - h^2 from the
+ *   rounded h; relu: [s > 0]), grad_enc[b,t] = sum_u ds, grad_pred[b,u] = sum_t ds.  dpx / dpy on padding are not
+ *   read; padding rows of grad_enc and grad_pred are zero.  The four gradients are accumulated in fp32 and written
+ *   once in bf16 (shapes of enc, pred, weight, bias); grad_bias may be NULL.  Bitwise deterministic for a given
+ *   chunk_cells: no float atomics.
+ * chunk_cells: cells (b, u, t) per pass through the scratch (h, dlogits and ds rows); 0 picks the largest multiple of
+ *   64 whose scratch fits in 256 MiB.  The workspace never grows with N T U V: per-cell lse, fp32 accumulators of
+ *   the four gradients, and the scratch.  The backward must get the forward's chunk_cells.
+ * Launches: the forward 2 per chunk; the backward 5 per chunk, 1 more, and one memset of the accumulators.  The
+ * calls are stream-ordered on options.stream without host synchronisation (graph-capturable).
+ * activation other than RNNT_B200_ACT_TANH / _RELU, hidden not a multiple of 16 in [16, 1024], alphabet_size < 2,
+ * blank_label outside [0, alphabet_size), chunk_cells < 0, minibatch, maxT or maxU < 1, maxU > 1024,
+ * minibatch * maxT * maxU >= 2^31, NULL pointers (flat_labels, px and dpx may be NULL when maxU == 1; bias and
+ * grad_bias may be NULL) and misaligned pointers are RNNT_STATUS_INVALID_VALUE before any device access; RNNT_CPU
+ * then returns RNNT_STATUS_EXECUTION_FAILED. */
+enum { RNNT_B200_ACT_TANH = 0, RNNT_B200_ACT_RELU = 1 };
+rnntStatus_t rnnt_b200_joiner_workspace_size(int maxT, int maxU, int minibatch, int hidden, int alphabet_size,
+                                             int chunk_cells, size_t* size_bytes);
+rnntStatus_t rnnt_b200_joiner_forward(int activation, const void* enc, const void* pred, const void* weight,
+                                      const void* bias, const int* flat_labels, const int* label_lengths,
+                                      const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                      int chunk_cells, float* px, float* py, void* workspace,
+                                      struct rnntOptions options);
+rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
+                                       const void* bias, const int* flat_labels, const int* label_lengths,
+                                       const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                       int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
+                                       void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
+                                       struct rnntOptions options);
+/* Kernels (memsets not counted) the last joiner call on this thread launched. */
+int rnnt_b200_joiner_last_launch_count(void);
+
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that
  * the last loss+gradient call left in `workspace`.  The reference checks their agreement in debug
  * builds (include/detail/cpu_rnnt.h:167-170); tests/test_gpu_round2.py does the same.  Synchronises. */

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "lib", "libwarprnnt.so")
-SOURCES = ["rnnt_entry.cu"]
+SOURCES = ["rnnt_entry.cu", "rnnt_joiner.cu"]
 # every source/header under csrc/ plus the public header: editing any of them marks the .so stale
 DEPS = sorted(f for f in os.listdir(SRC) if f.endswith((".cu", ".cuh", ".h"))) + \
        [os.path.join("..", "..", "include", "rnnt.h")]

@@ -1,0 +1,277 @@
+"""The RNN-T loss of a real joiner without the [N, T, U, V] logits (DESIGN.md §14).  icefall's ``Joiner``,
+torchaudio's ``RNNTJoiner`` and NeMo's ``RNNTJoint`` compute
+
+    logits[b, t, u, :] = weight @ act(enc[b, t] + pred[b, u]) + bias          act = tanh or relu
+
+with enc [N, T, H] and pred [N, U, H] already projected to the joiner width H.  ``joiner_log_probs`` reduces that
+joiner straight to the lattice factors of ``rnnt_lattice_loss`` on bf16 tensor cores, chunk by chunk, and its
+backward runs the contraction in reverse, so neither the logits nor their gradient ever exist:
+
+    px, py = joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens)   # px [N,S,T], py [N,S+1,T]
+    loss = joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens)
+    frames, scores = rnnt_lattice_forced_align(*joiner_log_probs(...), act_lens, label_lens)
+
+enc, pred, weight [V, H] (nn.Linear's layout) and bias [V] (or None) are bf16 CUDA tensors; pass a joiner's fp32
+master weights as ``weight.to(torch.bfloat16)`` and autograd carries the gradient back to them.
+"""
+import ctypes as C
+
+import torch
+from torch.autograd import Function
+from torch.nn import Module
+
+from . import warp_rnnt
+from ._checks import LengthCheck, check_contiguous, check_dim, check_type
+from .lattice import rnnt_lattice_loss
+
+_lib = warp_rnnt.lib()
+_P = C.c_void_p
+_lib.rnnt_b200_joiner_workspace_size.restype = C.c_int
+_lib.rnnt_b200_joiner_workspace_size.argtypes = [C.c_int] * 6 + [C.POINTER(C.c_size_t)]
+_lib.rnnt_b200_joiner_forward.restype = C.c_int
+_lib.rnnt_b200_joiner_forward.argtypes = [C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          _P, _P, _P, warp_rnnt.rnntOptions]
+_lib.rnnt_b200_joiner_backward.restype = C.c_int
+_lib.rnnt_b200_joiner_backward.argtypes = [C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
+                                           _P, _P, _P, _P, _P, _P, _P, warp_rnnt.rnntOptions]
+_lib.rnnt_b200_joiner_last_launch_count.restype = C.c_int
+
+RNNT_B200_ACT_TANH, RNNT_B200_ACT_RELU = 0, 1
+_ACTIVATIONS = {'tanh': RNNT_B200_ACT_TANH, 'relu': RNNT_B200_ACT_RELU}
+
+
+def activation_code(activation):
+    """The C-ABI's activation code for 'tanh' or 'relu'; ValueError otherwise."""
+    if activation not in _ACTIVATIONS:
+        raise ValueError("activation must be 'tanh' or 'relu', got %r" % (activation,))
+    return _ACTIVATIONS[activation]
+
+
+def _chunk(chunk_cells):
+    if chunk_cells is None:
+        return 0
+    if isinstance(chunk_cells, bool) or not isinstance(chunk_cells, int) or not 1 <= chunk_cells < 2 ** 31:
+        raise ValueError("chunk_cells must be None or an int in [1, 2^31), got %r" % (chunk_cells,))
+    return chunk_cells
+
+
+def workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells=None):
+    """Bytes of the joiner's workspace (include/rnnt.h rnnt_b200_joiner_workspace_size)."""
+    n = C.c_size_t(0)
+    st = _lib.rnnt_b200_joiner_workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, _chunk(chunk_cells),
+                                              C.byref(n))
+    if st != warp_rnnt.RNNT_STATUS_SUCCESS:
+        raise ValueError("rnnt_b200_joiner_workspace_size: " + warp_rnnt.status_string(st))
+    return n.value
+
+
+def last_launch_count():
+    """Kernels the last joiner call on this thread launched."""
+    return _lib.rnnt_b200_joiner_last_launch_count()
+
+
+def _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells):
+    """rnnt_loss's rules and exception types: ValueError for an option, a rank, a shape, an extent or a
+    non-contiguous tensor, TypeError for a dtype, RuntimeError for a CPU tensor or a second device.  Returns the
+    deferred T == max(act_lens), S == max(label_lens) check."""
+    activation_code(activation)
+    _chunk(chunk_cells)
+    for name, t in (("enc", enc), ("pred", pred), ("weight", weight), ("bias", bias)):
+        if t is not None and t.dtype is not torch.bfloat16:
+            raise TypeError("%s must be torch.bfloat16 (fp16 and fp32 are not supported), got %s" % (name, t.dtype))
+    check_type(labels, torch.int32, "labels")
+    check_type(act_lens, torch.int32, "lengths")
+    check_type(label_lens, torch.int32, "label_lengths")
+    for name, t, rank in (("enc", enc, 3), ("pred", pred, 3), ("weight", weight, 2), ("bias", bias, 1),
+                          ("labels", labels, 2), ("lengths", act_lens, 1), ("label_lengths", label_lens, 1)):
+        if t is not None:
+            check_contiguous(t, name)
+            check_dim(t, rank, name)
+    N, T, H = enc.shape
+    U = pred.shape[1]
+    V = weight.shape[0]
+    if pred.shape[0] != N or pred.shape[2] != H:
+        raise ValueError("pred must be [N, U, H] = [%d, U, %d], got %s" % (N, H, list(pred.shape)))
+    if weight.shape[1] != H:
+        raise ValueError("weight must be [V, H] with H = %d, got %s" % (H, list(weight.shape)))
+    if bias is not None and bias.shape[0] != V:
+        raise ValueError("bias must be [V] = [%d], got %s" % (V, list(bias.shape)))
+    if tuple(labels.shape) != (N, U - 1):
+        raise ValueError("labels must be [N, U-1] = %s, got %s" % ([N, U - 1], list(labels.shape)))
+    if act_lens.shape[0] != N:
+        raise ValueError("must have a length per example.")
+    if label_lens.shape[0] != N:
+        raise ValueError("must have a label length per example.")
+    if H % 16 != 0 or not 16 <= H <= 1024:
+        raise ValueError("the joiner width H must be a multiple of 16 in [16, 1024], got %d" % H)
+    if V < 2:
+        raise ValueError("the alphabet must have at least 2 symbols, got %d" % V)
+    if not 0 <= blank < V:
+        raise ValueError("blank must be in [0, %d), got %d" % (V, blank))
+    if N < 1 or T < 1 or U < 1:
+        raise ValueError("enc and pred must have at least one utterance, frame and context")
+    if U > 1024:
+        raise ValueError("U must be at most 1024, got %d" % U)
+    if N * T * U >= 2 ** 31:
+        raise ValueError("N * T * U must be below 2^31, got %d" % (N * T * U))
+    tensors = dict(pred=pred, weight=weight, bias=bias, labels=labels, act_lens=act_lens, label_lens=label_lens)
+    if not all(t.is_cuda for t in [enc] + [t for t in tensors.values() if t is not None]):
+        raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only; there is no CPU fallback")
+    warp_rnnt.require_same_device(enc, **tensors)
+    return LengthCheck(act_lens, label_lens, T, U)
+
+
+def _options(enc, U, blank):
+    opt = warp_rnnt.rnntOptions()
+    opt.loc = warp_rnnt.RNNT_GPU
+    opt.stream = torch.cuda.current_stream(enc.device).cuda_stream
+    opt.blank_label = blank
+    opt.maxT = enc.size(1)
+    opt.maxU = U
+    return opt
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None and t.numel() > 0 else None
+
+
+def gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px, py, blank, activation,
+                       chunk_cells=None, workspace=None):
+    """px [N, S, T] and py [N, S+1, T] (float32, every element written) from the joiner's inputs, checked by the
+    caller (include/rnnt.h rnnt_b200_joiner_forward).  Returns the workspace, which the backward reads."""
+    N, T, H = enc.shape
+    U, V = pred.shape[1], weight.shape[0]
+    with torch.cuda.device(enc.device):
+        need = workspace_size(T, U, N, H, V, chunk_cells)
+        if workspace is None or workspace.numel() < need:
+            workspace = torch.empty(need, dtype=torch.uint8, device=enc.device)
+        st = _lib.rnnt_b200_joiner_forward(activation_code(activation), enc.data_ptr(), pred.data_ptr(),
+                                           weight.data_ptr(), _ptr(bias), _ptr(labels), label_lens.data_ptr(),
+                                           act_lens.data_ptr(), H, V, N, _chunk(chunk_cells), _ptr(px),
+                                           py.data_ptr(), workspace.data_ptr(), _options(enc, U, blank))
+    if st != warp_rnnt.RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_joiner_forward failed: " + warp_rnnt.status_string(st))
+    return workspace
+
+
+def gpu_joiner_backward(enc, pred, weight, bias, labels, act_lens, label_lens, dpx, dpy, grad_enc, grad_pred,
+                        grad_weight, grad_bias, blank, activation, chunk_cells, workspace):
+    """The four bf16 gradients from dpx, dpy (float32, shaped as px, py) and the workspace of gpu_joiner_forward
+    with the same arguments (include/rnnt.h rnnt_b200_joiner_backward)."""
+    N, T, H = enc.shape
+    U, V = pred.shape[1], weight.shape[0]
+    with torch.cuda.device(enc.device):
+        st = _lib.rnnt_b200_joiner_backward(activation_code(activation), enc.data_ptr(), pred.data_ptr(),
+                                            weight.data_ptr(), _ptr(bias), _ptr(labels), label_lens.data_ptr(),
+                                            act_lens.data_ptr(), H, V, N, _chunk(chunk_cells), _ptr(dpx),
+                                            dpy.data_ptr(), grad_enc.data_ptr(), grad_pred.data_ptr(),
+                                            grad_weight.data_ptr(), _ptr(grad_bias), workspace.data_ptr(),
+                                            _options(enc, U, blank))
+    if st != warp_rnnt.RNNT_STATUS_SUCCESS:
+        raise RuntimeError("rnnt_b200_joiner_backward failed: " + warp_rnnt.status_string(st))
+
+
+class _JoinerLogProbs(Function):
+    """forward: 2 launches per chunk, px / py and the per-cell lse.  backward: 5 launches per chunk and 1 more,
+    from the lse the forward left in the workspace."""
+
+    @staticmethod
+    def forward(ctx, enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells):
+        length_check = _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
+                                     chunk_cells)
+        N, T, _ = enc.shape
+        S = pred.shape[1] - 1
+        px = torch.empty((N, S, T), dtype=torch.float32, device=enc.device)
+        py = torch.empty((N, S + 1, T), dtype=torch.float32, device=enc.device)
+        ws = gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px, py, blank, activation,
+                                chunk_cells)
+        length_check.finish()
+        ctx.save_for_backward(enc, pred, weight, bias, labels, act_lens, label_lens)
+        ctx.workspace = ws
+        ctx.args = (blank, activation, chunk_cells)
+        return px, py
+
+    @staticmethod
+    def backward(ctx, dpx, dpy):
+        enc, pred, weight, bias, labels, act_lens, label_lens = ctx.saved_tensors
+        blank, activation, chunk_cells = ctx.args
+        N, T, _ = enc.shape
+        S = pred.shape[1] - 1
+        dpx = (torch.zeros((N, S, T), dtype=torch.float32, device=enc.device) if dpx is None
+               else dpx.to(torch.float32).contiguous())
+        dpy = (torch.zeros((N, S + 1, T), dtype=torch.float32, device=enc.device) if dpy is None
+               else dpy.to(torch.float32).contiguous())
+        grad_enc, grad_pred, grad_weight = torch.empty_like(enc), torch.empty_like(pred), torch.empty_like(weight)
+        grad_bias = torch.empty_like(bias) if bias is not None else None
+        gpu_joiner_backward(enc, pred, weight, bias, labels, act_lens, label_lens, dpx, dpy, grad_enc, grad_pred,
+                            grad_weight, grad_bias, blank, activation, chunk_cells, ctx.workspace)
+        need = ctx.needs_input_grad
+        return (grad_enc if need[0] else None, grad_pred if need[1] else None, grad_weight if need[2] else None,
+                grad_bias if bias is not None and need[3] else None, None, None, None, None, None, None)
+
+
+def joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blank=0, *, activation='tanh',
+                     chunk_cells=None):
+    """The lattice factors of the joiner  logits = weight act(enc[b,t] + pred[b,u]) + bias,  without the logits.
+
+    enc [N, T, H], pred [N, U, H], weight [V, H], bias [V] or None: bf16, contiguous, on one CUDA device, with
+    H % 16 == 0, 16 <= H <= 1024, V >= 2, U <= 1024 and N T U < 2^31.  labels [N, U-1], act_lens and label_lens [N]
+    are int32, with T == max(act_lens) and U == max(label_lens) + 1 (checked after the kernels are queued).
+
+    Returns float32 px [N, U-1, T] (label s at frame t) and py [N, U, T] (blank at (t, s)), rnnt_lattice_loss's
+    orientation: px[b,s,t] = logit_{labels[b,s]} - lse and py[b,s,t] = logit_blank - lse, -inf on padding.  The
+    hidden activation is h = round_bf16(act(fp32(enc) + fp32(pred))) with act tanhf or relu: one rounding fewer than
+    a bf16 eager joiner, which also rounds the sum.  The logits are h weight^T + bias in fp32 and lse their fp32
+    logsumexp.  A label outside [0, V) gives px = NaN on its row.  Both outputs are differentiable: the
+    backward returns bf16 gradients of enc, pred, weight and bias, accumulated in fp32 and bitwise deterministic for
+    a given chunk_cells.
+
+    chunk_cells: cells per pass through the scratch; None keeps the scratch within 256 MiB."""
+    return _JoinerLogProbs.apply(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
+                                 chunk_cells)
+
+
+def _delay(px, act_lens, delay_penalty):
+    """px + delay_penalty ((T_b - 1) / 2 - t): rnnt_loss's delay-penalised label factors."""
+    T = px.shape[2]
+    t = torch.arange(T, device=px.device, dtype=torch.float32)
+    tb = act_lens.to(torch.float32).clamp(1, T).unsqueeze(1)
+    return px + (delay_penalty * ((tb - 1) * 0.5 - t)).unsqueeze(1)
+
+
+def joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank=0, reduction='mean', *,
+                     activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+    """RNN-T loss of the joiner  logits = weight act(enc[b,t] + pred[b,u]) + bias  (see joiner_log_probs), without
+    the [N, T, U, V] logits or their gradient:
+
+        rnnt_lattice_loss(px + delay_penalty ((T_b - 1)/2 - t), py, act_lens, label_lens, reduction, rnnt_type)
+
+    on (px, py) = joiner_log_probs(...).  reduction, rnnt_type and delay_penalty are rnnt_loss's."""
+    warp_rnnt.rnnt_type_code(rnnt_type)
+    warp_rnnt.lattice_options(delay_penalty)
+    if reduction not in ('none', 'sum', 'mean'):
+        raise ValueError("reduction must be 'none', 'sum' or 'mean'")
+    px, py = joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation=activation)
+    if delay_penalty:
+        px = _delay(px, act_lens, float(delay_penalty))
+    return rnnt_lattice_loss(px, py, act_lens, label_lens, reduction, rnnt_type=rnnt_type)
+
+
+class JoinerRNNTLoss(Module):
+    """Module form of joiner_rnnt_loss: JoinerRNNTLoss(blank=0, reduction='mean', *, activation='tanh',
+    rnnt_type='regular', delay_penalty=0.0); forward(enc, pred, weight, bias, labels, act_lens, label_lens)."""
+
+    def __init__(self, blank=0, reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+        super().__init__()
+        activation_code(activation)
+        warp_rnnt.rnnt_type_code(rnnt_type)
+        warp_rnnt.lattice_options(delay_penalty)
+        if reduction not in ('none', 'sum', 'mean'):
+            raise ValueError("reduction must be 'none', 'sum' or 'mean'")
+        self.blank, self.reduction = blank, reduction
+        self.activation, self.rnnt_type, self.delay_penalty = activation, rnnt_type, delay_penalty
+
+    def forward(self, enc, pred, weight, bias, labels, act_lens, label_lens):
+        return joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, self.blank, self.reduction,
+                                activation=self.activation, rnnt_type=self.rnnt_type,
+                                delay_penalty=self.delay_penalty)
