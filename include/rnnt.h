@@ -686,7 +686,37 @@ rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const vo
                                        int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
                                        void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
                                        struct rnntOptions options);
-/* Kernels (memsets not counted) the last joiner call on this thread launched. */
+
+/* Pruned fused joiner (DESIGN.md §15): the fused joiner's factors on the pruned lattice of rnnt_b200_pruned_*, without
+ * the [N, T, s_range, V] logits.  Arguments as the fused joiner's, plus ranges [N, maxT] (int32 device pointer) and
+ * s_range = R >= 1.  Row (b, t, r), r < R, stands for lattice cell (t, u = ranges[b,t] + r), u formed without
+ * overflow for any int32 window start; the row is valid when t < T_b and 0 <= u <= S_b (R > maxU is allowed).
+ * forward: px [N, maxU-1, maxT] and py [N, maxU, maxT] in rnnt_b200_joiner_forward's layout; on a valid row's cell
+ *   the fused joiner's values, every other element -inf (every element is written).  Padded rows of enc and pred,
+ *   and pred rows no valid row selects, are not read.  The workspace keeps one fp32 lse per row.
+ * backward: the fused joiner's gradients over the valid rows only: dpx / dpy are read only at the cells valid rows
+ *   cover.  grad_enc[b,t] sums its rows in r order, grad_pred[b,u] the rows selecting u in t order; bf16, fp32
+ *   accumulation, bitwise deterministic for a given chunk_cells.  With s_range = maxU and ranges = 0 both halves are
+ *   bitwise the fused joiner's.
+ * chunk_cells counts rows (b, t, r).  The workspace holds the per-row lse (4 N maxT R bytes), the same fp32
+ * accumulators (grad_pred's stays N maxU hidden) and scratch as the fused joiner's.
+ * Launches: the forward 1 (the -inf fill) + 2 per chunk; the backward 5 per chunk, 1 more, and one memset.
+ * The fused joiner's rules, NULL ranges, s_range < 1 and minibatch * maxT * s_range >= 2^31 are
+ * RNNT_STATUS_INVALID_VALUE before any device access. */
+rnntStatus_t rnnt_b200_pruned_joiner_workspace_size(int maxT, int maxU, int s_range, int minibatch, int hidden,
+                                                    int alphabet_size, int chunk_cells, size_t* size_bytes);
+rnntStatus_t rnnt_b200_pruned_joiner_forward(int activation, const void* enc, const void* pred, const void* weight,
+                                             const void* bias, const int* flat_labels, const int* label_lengths,
+                                             const int* input_lengths, const int* ranges, int s_range, int hidden,
+                                             int alphabet_size, int minibatch, int chunk_cells, float* px, float* py,
+                                             void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
+                                              const void* bias, const int* flat_labels, const int* label_lengths,
+                                              const int* input_lengths, const int* ranges, int s_range, int hidden,
+                                              int alphabet_size, int minibatch, int chunk_cells, const float* dpx,
+                                              const float* dpy, void* grad_enc, void* grad_pred, void* grad_weight,
+                                              void* grad_bias, void* workspace, struct rnntOptions options);
+/* Kernels (memsets not counted) the last fused or pruned joiner call on this thread launched. */
 int rnnt_b200_joiner_last_launch_count(void);
 
 /* Debug / test hook: forward and backward log-likelihoods (natural log, as doubles on the host) that

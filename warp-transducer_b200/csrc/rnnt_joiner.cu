@@ -1,4 +1,5 @@
-// C-ABI of the fused joiner (include/rnnt.h, DESIGN.md §14): workspace sizing, argument rules and the chunk loop.
+// C-ABI of the fused joiner (include/rnnt.h, DESIGN.md §14) and of the pruned fused joiner (§15): workspace sizing,
+// argument rules and the chunk loop, shared by both; the pruned calls run the same loop over N T R window rows.
 // A translation unit of its own, so the kernels of rnnt_entry.cu compile exactly as they did without it.
 #include <cuda_runtime.h>
 
@@ -42,12 +43,18 @@ bool extents_ok(int maxT, int maxU, int minibatch, int hidden, int alphabet_size
     return chunk_cells >= 0;
 }
 
-Plan plan(int maxT, int maxU, int minibatch, int hidden, int alphabet_size, int chunk_cells) {
+// The pruned rules beyond extents_ok: a window of s_range >= 1 rows per frame and N T R < 2^31.
+bool window_ok(int maxT, int minibatch, int s_range) {
+    return s_range >= 1 && (long long)minibatch * maxT * s_range < (1LL << 31);
+}
+
+// rows_per_frame: maxU for the dense grid (b, u, t), s_range for the pruned rows (b, r, t).
+Plan plan(int maxT, int maxU, int minibatch, int hidden, int alphabet_size, int chunk_cells, int rows_per_frame) {
     Plan p;
     p.N = minibatch, p.T = maxT, p.U = maxU, p.H = hidden, p.V = alphabet_size;
     p.Hp = (int)up(hidden + 1, TILE);           // column H of h is the constant 1 of dbias
     p.Vp = (int)up(alphabet_size, TILE);
-    p.cells = minibatch * maxT * maxU;
+    p.cells = minibatch * maxT * rows_per_frame;
     const size_t row = (size_t)p.Hp * 2 + (size_t)p.Vp * 2 + (size_t)p.H * 4;   // h, dlogits, ds
     if (chunk_cells == 0) {   // whole waves of 128-row CTAs where the cap allows
         const size_t wave = (size_t)kMaxRows * kSMs;
@@ -104,8 +111,17 @@ size_t logits_smem(int hidden) {
 }
 constexpr size_t kPairSmem = (size_t)2 * PAIR_STAGES * TILE_ELEMS * 2;
 
-// The dynamic shared-memory opt-in of every kernel, for the largest call, once per device: after one call on a
-// device, calls made during CUDA-graph capture make no attribute calls.
+template <bool PRUNED>
+bool allow_smem(cudaFuncAttribute attr, int big, int small) {
+    return cudaFuncSetAttribute(joiner_lse_kernel<128, PRUNED>, attr, big) == cudaSuccess &&
+           cudaFuncSetAttribute(joiner_dlogits_kernel<128, PRUNED>, attr, big) == cudaSuccess &&
+           cudaFuncSetAttribute(joiner_lse_kernel<64, PRUNED>, attr, small) == cudaSuccess &&
+           cudaFuncSetAttribute(joiner_dlogits_kernel<64, PRUNED>, attr, small) == cudaSuccess &&
+           cudaFuncSetAttribute(joiner_ds_kernel<PRUNED>, attr, (int)kPairSmem) == cudaSuccess;
+}
+
+// The dynamic shared-memory opt-in of every kernel, dense and pruned, for the largest call, once per device: after
+// one call on a device, calls made during CUDA-graph capture make no attribute calls.
 bool allow_smem() {
     constexpr int kMaxDevices = 64;
     static std::atomic<bool> done[kMaxDevices];
@@ -114,11 +130,7 @@ bool allow_smem() {
     if (dev < kMaxDevices && done[dev].load()) return true;
     const auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
     const int big = (int)logits_smem(640), small = (int)logits_smem(1024);   // the largest of each tile height
-    const bool ok = cudaFuncSetAttribute(joiner_lse_kernel<128>, attr, big) == cudaSuccess &&
-                    cudaFuncSetAttribute(joiner_dlogits_kernel<128>, attr, big) == cudaSuccess &&
-                    cudaFuncSetAttribute(joiner_lse_kernel<64>, attr, small) == cudaSuccess &&
-                    cudaFuncSetAttribute(joiner_dlogits_kernel<64>, attr, small) == cudaSuccess &&
-                    cudaFuncSetAttribute(joiner_ds_kernel, attr, (int)kPairSmem) == cudaSuccess &&
+    const bool ok = allow_smem<false>(attr, big, small) && allow_smem<true>(attr, big, small) &&
                     cudaFuncSetAttribute(joiner_dw_kernel, attr, (int)kPairSmem) == cudaSuccess;
     if (ok && dev < kMaxDevices) done[dev].store(true);
     return ok;
@@ -133,36 +145,21 @@ rnntStatus_t launched() {
     return cudaGetLastError() == cudaSuccess ? RNNT_STATUS_SUCCESS : RNNT_STATUS_EXECUTION_FAILED;
 }
 
-void launch_h(const Geo& g, int act, const bf16* enc, const bf16* pred, bf16* h, int rows, cudaStream_t s) {
-    joiner_h_kernel<<<blocks((long long)rows * (g.Hp / 8), 256), 256, 0, s>>>(g, act, enc, pred, h, rows);
+template <bool PRUNED>
+void launch_h(const Geo& g, int act, const bf16* enc, const bf16* pred, bf16* h, int rows, cudaStream_t s,
+              const Window& w) {
+    joiner_h_kernel<PRUNED><<<blocks((long long)rows * (g.Hp / 8), 256), 256, 0, s>>>(g, act, enc, pred, h, rows, w);
     ++g_joiner_launches;
 }
 
-}  // namespace
-
-extern "C" {
-
-rnntStatus_t rnnt_b200_joiner_workspace_size(int maxT, int maxU, int minibatch, int hidden, int alphabet_size,
-                                             int chunk_cells, size_t* size_bytes) {
-    if (!size_bytes || !extents_ok(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells))
-        return RNNT_STATUS_INVALID_VALUE;
-    *size_bytes = plan(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells).bytes;
-    return RNNT_STATUS_SUCCESS;
-}
-
-rnntStatus_t rnnt_b200_joiner_forward(int activation, const void* enc, const void* pred, const void* weight,
-                                      const void* bias, const int* flat_labels, const int* label_lengths,
-                                      const int* input_lengths, int hidden, int alphabet_size, int minibatch,
-                                      int chunk_cells, float* px, float* py, void* workspace,
-                                      struct rnntOptions options) {
-    g_joiner_launches = 0;
-    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
-                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
-    if (st != RNNT_STATUS_SUCCESS) return st;
-    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
-    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
-
-    const Plan p = plan(options.maxT, options.maxU, minibatch, hidden, alphabet_size, chunk_cells);
+// The forward chunk loop of both entries (pruned: after filling px and py with -inf).
+template <bool PRUNED>
+rnntStatus_t forward(int activation, const void* enc, const void* pred, const void* weight, const void* bias,
+                     const int* flat_labels, const int* label_lengths, const int* input_lengths, int hidden,
+                     int alphabet_size, int minibatch, int chunk_cells, float* px, float* py, void* workspace,
+                     const rnntOptions& options, const Window& w) {
+    const Plan p = plan(options.maxT, options.maxU, minibatch, hidden, alphabet_size, chunk_cells,
+                        PRUNED ? w.R : options.maxU);
     char* ws = static_cast<char*>(workspace);
     float* lse = reinterpret_cast<float*>(ws + p.lse);
     bf16* h = reinterpret_cast<bf16*>(ws + p.h);
@@ -173,35 +170,35 @@ rnntStatus_t rnnt_b200_joiner_forward(int activation, const void* enc, const voi
     Geo g = geo(p, options.blank_label, flat_labels, label_lengths, input_lengths);
     const bf16* W = static_cast<const bf16*>(weight);
     const bf16* B = static_cast<const bf16*>(bias);
+    if (PRUNED) {
+        const long long npx = (long long)p.N * (p.U - 1) * p.T, npy = (long long)p.N * p.U * p.T;
+        joiner_fill_kernel<<<blocks(npx + npy, 256), 256, 0, s>>>(px, npx, py, npy);
+        ++g_joiner_launches;
+    }
     for (int c0 = 0; c0 < p.cells; c0 += p.chunk) {
         g.c0 = c0;
         g.m = p.cells - c0 < p.chunk ? p.cells - c0 : p.chunk;
         const int tiles = (g.m + bm - 1) / bm;
-        launch_h(g, activation, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred), h, tiles * bm, s);
+        launch_h<PRUNED>(g, activation, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred), h, tiles * bm,
+                         s, w);
         if (bm == 128)
-            joiner_lse_kernel<128><<<tiles, 256, smem, s>>>(g, h, W, B, lse, px, py);
+            joiner_lse_kernel<128, PRUNED><<<tiles, 256, smem, s>>>(g, h, W, B, lse, px, py, w);
         else
-            joiner_lse_kernel<64><<<tiles, 128, smem, s>>>(g, h, W, B, lse, px, py);
+            joiner_lse_kernel<64, PRUNED><<<tiles, 128, smem, s>>>(g, h, W, B, lse, px, py, w);
         ++g_joiner_launches;
     }
     return launched();
 }
 
-rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
-                                       const void* bias, const int* flat_labels, const int* label_lengths,
-                                       const int* input_lengths, int hidden, int alphabet_size, int minibatch,
-                                       int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
-                                       void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
-                                       struct rnntOptions options) {
-    g_joiner_launches = 0;
-    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
-                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
-    if (st != RNNT_STATUS_SUCCESS) return st;
-    if (!dpy || (!dpx && options.maxU > 1) || !grad_enc || !grad_pred || !grad_weight)
-        return RNNT_STATUS_INVALID_VALUE;
-    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
-
-    const Plan p = plan(options.maxT, options.maxU, minibatch, hidden, alphabet_size, chunk_cells);
+// The backward chunk loop of both entries.
+template <bool PRUNED>
+rnntStatus_t backward(int activation, const void* enc, const void* pred, const void* weight, const void* bias,
+                      const int* flat_labels, const int* label_lengths, const int* input_lengths, int hidden,
+                      int alphabet_size, int minibatch, int chunk_cells, const float* dpx, const float* dpy,
+                      void* grad_enc, void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
+                      const rnntOptions& options, const Window& w) {
+    const Plan p = plan(options.maxT, options.maxU, minibatch, hidden, alphabet_size, chunk_cells,
+                        PRUNED ? w.R : options.maxU);
     char* ws = static_cast<char*>(workspace);
     const float* lse = reinterpret_cast<const float*>(ws + p.lse);
     float* denc = reinterpret_cast<float*>(ws + p.denc);
@@ -219,22 +216,26 @@ rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const vo
     if (cudaMemsetAsync(ws + p.denc, 0, p.h - p.denc, s) != cudaSuccess) return RNNT_STATUS_EXECUTION_FAILED;
 
     Geo g = geo(p, options.blank_label, flat_labels, label_lengths, input_lengths);
+    const int per_b = PRUNED ? w.R : p.U;   // grid rows of T cells per utterance
     for (int c0 = 0; c0 < p.cells; c0 += p.chunk) {
         g.c0 = c0;
         g.m = p.cells - c0 < p.chunk ? p.cells - c0 : p.chunk;
         const int ltiles = (g.m + bm - 1) / bm, tiles = (g.m + TILE - 1) / TILE;
-        launch_h(g, activation, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred), h, ltiles * bm, s);
+        launch_h<PRUNED>(g, activation, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred), h,
+                         ltiles * bm, s, w);
         if (bm == 128)
-            joiner_dlogits_kernel<128><<<ltiles, 256, smem, s>>>(g, h, W, static_cast<const bf16*>(bias), lse, dpx,
-                                                                 dpy, dlog);
+            joiner_dlogits_kernel<128, PRUNED><<<ltiles, 256, smem, s>>>(g, h, W, static_cast<const bf16*>(bias), lse,
+                                                                         dpx, dpy, dlog, w);
         else
-            joiner_dlogits_kernel<64><<<ltiles, 128, smem, s>>>(g, h, W, static_cast<const bf16*>(bias), lse, dpx,
-                                                                dpy, dlog);
-        joiner_ds_kernel<<<dim3(tiles, (p.H + TILE - 1) / TILE), THREADS, kPairSmem, s>>>(g, activation, dlog, W, h,
-                                                                                          ds);
+            joiner_dlogits_kernel<64, PRUNED><<<ltiles, 128, smem, s>>>(g, h, W, static_cast<const bf16*>(bias), lse,
+                                                                        dpx, dpy, dlog, w);
+        joiner_ds_kernel<PRUNED><<<dim3(tiles, (p.H + TILE - 1) / TILE), THREADS, kPairSmem, s>>>(g, activation, dlog,
+                                                                                                  W, h, ds, w);
         const int bu_lo = c0 / p.T, bu_hi = (c0 + g.m - 1) / p.T;
-        const long long red = ((long long)(bu_hi - bu_lo + 1) + (long long)(bu_hi / p.U - bu_lo / p.U + 1) * p.T) * p.H;
-        joiner_reduce_kernel<<<blocks(red, 256), 256, 0, s>>>(g, ds, denc, dpred);
+        const long long b_n = bu_hi / per_b - bu_lo / per_b + 1;
+        // dense: one thread per (b, u) row and per (b, t) of the chunk; pruned: per (b, u) and (b, t) of its b
+        const long long red = (PRUNED ? b_n * p.U : (long long)(bu_hi - bu_lo + 1)) * p.H + b_n * p.T * p.H;
+        joiner_reduce_kernel<PRUNED><<<blocks(red, 256), 256, 0, s>>>(g, ds, denc, dpred, w);
         const int per = (tiles + p.slabs - 1) / p.slabs;
         joiner_dw_kernel<<<dim3(p.Vp / TILE, p.Hp / TILE, (tiles + per - 1) / per), THREADS, kPairSmem, s>>>(
             g, dlog, h, dw, tiles, per);
@@ -246,6 +247,95 @@ rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const vo
                                                        static_cast<bf16*>(grad_pred));
     ++g_joiner_launches;
     return launched();
+}
+
+}  // namespace
+
+extern "C" {
+
+rnntStatus_t rnnt_b200_joiner_workspace_size(int maxT, int maxU, int minibatch, int hidden, int alphabet_size,
+                                             int chunk_cells, size_t* size_bytes) {
+    if (!size_bytes || !extents_ok(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells))
+        return RNNT_STATUS_INVALID_VALUE;
+    *size_bytes = plan(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells, maxU).bytes;
+    return RNNT_STATUS_SUCCESS;
+}
+
+rnntStatus_t rnnt_b200_joiner_forward(int activation, const void* enc, const void* pred, const void* weight,
+                                      const void* bias, const int* flat_labels, const int* label_lengths,
+                                      const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                      int chunk_cells, float* px, float* py, void* workspace,
+                                      struct rnntOptions options) {
+    g_joiner_launches = 0;
+    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
+                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
+    if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
+    return forward<false>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
+                          alphabet_size, minibatch, chunk_cells, px, py, workspace, options, Window{nullptr, 0});
+}
+
+rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
+                                       const void* bias, const int* flat_labels, const int* label_lengths,
+                                       const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                       int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
+                                       void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
+                                       struct rnntOptions options) {
+    g_joiner_launches = 0;
+    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
+                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
+    if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!dpy || (!dpx && options.maxU > 1) || !grad_enc || !grad_pred || !grad_weight)
+        return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
+    return backward<false>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
+                           alphabet_size, minibatch, chunk_cells, dpx, dpy, grad_enc, grad_pred, grad_weight,
+                           grad_bias, workspace, options, Window{nullptr, 0});
+}
+
+rnntStatus_t rnnt_b200_pruned_joiner_workspace_size(int maxT, int maxU, int s_range, int minibatch, int hidden,
+                                                    int alphabet_size, int chunk_cells, size_t* size_bytes) {
+    if (!size_bytes || !extents_ok(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells) ||
+        !window_ok(maxT, minibatch, s_range))
+        return RNNT_STATUS_INVALID_VALUE;
+    *size_bytes = plan(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells, s_range).bytes;
+    return RNNT_STATUS_SUCCESS;
+}
+
+rnntStatus_t rnnt_b200_pruned_joiner_forward(int activation, const void* enc, const void* pred, const void* weight,
+                                             const void* bias, const int* flat_labels, const int* label_lengths,
+                                             const int* input_lengths, const int* ranges, int s_range, int hidden,
+                                             int alphabet_size, int minibatch, int chunk_cells, float* px, float* py,
+                                             void* workspace, struct rnntOptions options) {
+    g_joiner_launches = 0;
+    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
+                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
+    if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!ranges || !window_ok(options.maxT, minibatch, s_range)) return RNNT_STATUS_INVALID_VALUE;
+    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
+    return forward<true>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
+                         alphabet_size, minibatch, chunk_cells, px, py, workspace, options, Window{ranges, s_range});
+}
+
+rnntStatus_t rnnt_b200_pruned_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
+                                              const void* bias, const int* flat_labels, const int* label_lengths,
+                                              const int* input_lengths, const int* ranges, int s_range, int hidden,
+                                              int alphabet_size, int minibatch, int chunk_cells, const float* dpx,
+                                              const float* dpy, void* grad_enc, void* grad_pred, void* grad_weight,
+                                              void* grad_bias, void* workspace, struct rnntOptions options) {
+    g_joiner_launches = 0;
+    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
+                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
+    if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!ranges || !window_ok(options.maxT, minibatch, s_range)) return RNNT_STATUS_INVALID_VALUE;
+    if (!dpy || (!dpx && options.maxU > 1) || !grad_enc || !grad_pred || !grad_weight)
+        return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
+    return backward<true>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
+                          alphabet_size, minibatch, chunk_cells, dpx, dpy, grad_enc, grad_pred, grad_weight,
+                          grad_bias, workspace, options, Window{ranges, s_range});
 }
 
 int rnnt_b200_joiner_last_launch_count(void) { return g_joiner_launches; }

@@ -4,6 +4,8 @@
 // t fastest; a chunk of m cells is m scratch rows.  Every contraction is a 64x64 output tile per CTA, 4 warps of
 // 32x32, mma.sync.m16n8k16 bf16 with fp32 accumulators, operands staged through 64x64 swizzled shared-memory tiles
 // by cp.async (zero-filled past the operand's extent) and read with ldmatrix (.trans for MN-major operands).
+// The pruned joiner (DESIGN.md §15) runs the same kernels with PRUNED = true over the rows (b, r, t), t fastest, of
+// the windows: row (b, r, t) is cell (t, ranges[b,t] + r), and px / py are written at the cell's dense index.
 #pragma once
 #include <cuda_bf16.h>
 #include <math.h>
@@ -31,25 +33,48 @@ struct Geo {
     const int* labels;                // [N, S]
 };
 
+// The pruned window: rows (b, r, t) with r < R stand for cells (t, ranges[b,t] + r).  Dense calls pass {nullptr, 0}
+// and never read it.
+struct Window {
+    const int* ranges;   // [N, T]
+    int R;
+};
+
 struct Cell {
     int b, u, t;
-    bool valid;       // t < T_b and u <= S_b: the cell has a blank factor
-    bool has_label;   // t < T_b and u < S_b: it also has a label factor
+    bool valid;       // t < T_b and 0 <= u <= S_b: the cell has a blank factor
+    bool has_label;   // t < T_b and 0 <= u < S_b: it also has a label factor
+    int dense;        // (b * U + u) * T + t, the cell's py index (px: (b * S + u) * T + t); meaningful when valid.
+                      // The row's lse index is its grid index c0 + r (dense: the same).
 };
 
 __device__ __forceinline__ int clampi(int x, int lo, int hi) { return x < lo ? lo : (x > hi ? hi : x); }
 
-__device__ __forceinline__ Cell decode(const Geo& g, int r) {
-    Cell k{0, 0, 0, false, false};
+// Row r of the chunk.  Dense: grid index (b, u, t).  PRUNED: grid index (b, r', t), u = ranges[b,t] + r' formed in
+// 64 bits, so any int32 window start is well defined; rows whose u falls outside [0, S_b] are padding.
+template <bool PRUNED = false>
+__device__ __forceinline__ Cell decode(const Geo& g, int r, const Window& w = Window{nullptr, 0}) {
+    Cell k{0, 0, 0, false, false, 0};
     if (r >= g.m) return k;
     const int c = g.c0 + r;
     k.t = c % g.T;
     const int bu = c / g.T;
-    k.u = bu % g.U;
-    k.b = bu / g.U;
-    const int Tb = clampi(g.xlen[k.b], 1, g.T), Sb = clampi(g.ylen[k.b], 0, g.S);
-    k.valid = k.t < Tb && k.u <= Sb;
-    k.has_label = k.t < Tb && k.u < Sb;
+    if constexpr (!PRUNED) {
+        k.u = bu % g.U;
+        k.b = bu / g.U;
+        const int Tb = clampi(g.xlen[k.b], 1, g.T), Sb = clampi(g.ylen[k.b], 0, g.S);
+        k.valid = k.t < Tb && k.u <= Sb;
+        k.has_label = k.t < Tb && k.u < Sb;
+        k.dense = c;
+    } else {
+        k.b = bu / w.R;
+        const long long u = (long long)w.ranges[(size_t)k.b * g.T + k.t] + bu % w.R;
+        const int Tb = clampi(g.xlen[k.b], 1, g.T), Sb = clampi(g.ylen[k.b], 0, g.S);
+        k.valid = k.t < Tb && u >= 0 && u <= Sb;
+        k.has_label = k.valid && u < Sb;
+        k.u = k.valid ? (int)u : 0;
+        k.dense = (k.b * g.U + k.u) * g.T + k.t;
+    }
     return k;
 }
 
@@ -163,26 +188,43 @@ __device__ __forceinline__ void mma_tile(Acc& acc, const bf16* As, const bf16* B
 }
 
 // Per-row metadata of an R-row tile of the chunk, in shared memory.
-template <int R = TILE>
-struct RowInfo {
+template <int R, bool PRUNED>
+struct RowPy {
+    int pyi[R];     // py index (b, u, t) of a valid pruned row
+};
+template <int R>
+struct RowPy<R, false> {};   // a dense row's py index is its cell index
+
+template <int R = TILE, bool PRUNED = false>
+struct RowInfo : RowPy<R, PRUNED> {
     int flag[R];    // bit 0 valid, bit 1 has_label
     int label[R];   // labels[b, u] where has_label (compared with columns, never used as an address)
-    int cell[R];    // py index (b, u, t) = the cell index
-    int pxi[R];     // px index (b, u, t) where u < S, else -1
+    int cell[R];    // the row's grid index: its lse index, and (dense) its py index (b, u, t)
+    int pxi[R];     // px index (b, u, t) where u < S (PRUNED: where has_label), else -1
+
+    __device__ __forceinline__ int py(int i) const {
+        if constexpr (PRUNED) return this->pyi[i];
+        else return cell[i];
+    }
 };
 
 // Fills ri for rows r0 .. r0 + R - 1; returns whether any of them is a valid cell.
-template <int R>
-__device__ __forceinline__ int load_rows(const Geo& g, int r0, RowInfo<R>& ri, int* any) {
+template <int R, bool PRUNED>
+__device__ __forceinline__ int load_rows(const Geo& g, const Window& w, int r0, RowInfo<R, PRUNED>& ri, int* any) {
     if (threadIdx.x == 0) *any = 0;
     __syncthreads();
     if (threadIdx.x < R) {
         const int i = threadIdx.x;
-        const Cell k = decode(g, r0 + i);
+        const Cell k = decode<PRUNED>(g, r0 + i, w);
         ri.flag[i] = (k.valid ? 1 : 0) | (k.has_label ? 2 : 0);
         ri.label[i] = k.has_label ? g.labels[(size_t)k.b * g.S + k.u] : 0;
         ri.cell[i] = g.c0 + r0 + i;
-        ri.pxi[i] = (r0 + i < g.m && k.u < g.S) ? (k.b * g.S + k.u) * g.T + k.t : -1;
+        if constexpr (PRUNED) {
+            ri.pxi[i] = k.has_label ? (k.b * g.S + k.u) * g.T + k.t : -1;
+            ri.pyi[i] = k.dense;
+        } else {
+            ri.pxi[i] = (r0 + i < g.m && k.u < g.S) ? (k.b * g.S + k.u) * g.T + k.t : -1;
+        }
         if (k.valid) *any = 1;
     }
     __syncthreads();
@@ -192,9 +234,10 @@ __device__ __forceinline__ int load_rows(const Geo& g, int r0, RowInfo<R>& ri, i
 // h[r, :] = round_bf16(act(enc[b,t] + pred[b,u])) for a valid cell, 0 for padding and rows past the chunk; column H
 // is 1 (the dW contraction then yields dbias as its column H), columns H+1 .. Hp-1 are 0.  Padded rows of enc and
 // pred are never read.
+template <bool PRUNED>
 __global__ void __launch_bounds__(256) joiner_h_kernel(Geo g, int act, const bf16* __restrict__ enc,
                                                        const bf16* __restrict__ pred, bf16* __restrict__ h,
-                                                       int rows) {
+                                                       int rows, Window w) {
     const int groups = g.Hp / 8;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < (long long)rows * groups;
          i += (long long)gridDim.x * blockDim.x) {
@@ -203,7 +246,7 @@ __global__ void __launch_bounds__(256) joiner_h_kernel(Geo g, int act, const bf1
 #pragma unroll
     for (int e = 0; e < 8; ++e) out[e] = __float2bfloat16_rn(0.f);
     if (k0 < g.H) {
-        const Cell k = decode(g, r);
+        const Cell k = decode<PRUNED>(g, r, w);
         if (k.valid) {
             const uint4 ev = *reinterpret_cast<const uint4*>(enc + ((size_t)k.b * g.T + k.t) * g.H + k0);
             const uint4 pv = *reinterpret_cast<const uint4*>(pred + ((size_t)k.b * g.U + k.u) * g.H + k0);
@@ -226,16 +269,17 @@ __global__ void __launch_bounds__(256) joiner_h_kernel(Geo g, int act, const bf1
 // The logits GEMM of one BM-row tile of h (BM = 64 or 128, BM / 32 x 2 warps) against every column of W,
 // row-stationary: the tile's h rows stay in shared memory, W streams through in 64 x 64 tiles, each shared by all the
 // rows.  BWD = false: online max / sum over the columns, the blank and label logits captured, then lse, px and py.
-// BWD = true: dlogits from the forward's lse and the incoming dpx, dpy.
-template <bool BWD, int BM>
+// BWD = true: dlogits from the forward's lse and the incoming dpx, dpy.  PRUNED: px / py are written (and dpx / dpy
+// read) at valid rows only; the caller filled px / py with -inf beforehand.
+template <bool BWD, int BM, bool PRUNED>
 __device__ __forceinline__ void logits_tile(const Geo& g, const bf16* __restrict__ h, const bf16* __restrict__ W,
                                             const bf16* __restrict__ bias, float* __restrict__ lse,
                                             float* __restrict__ px, float* __restrict__ py,
                                             const float* __restrict__ dpx, const float* __restrict__ dpy,
-                                            bf16* __restrict__ dlog) {
+                                            bf16* __restrict__ dlog, const Window& w) {
     constexpr int NT = BM * 2, RT = BM / TILE;   // threads; 64-row h tiles per k block
     extern __shared__ __align__(128) unsigned char smem_raw[];   // BM h rows, then STAGES W tiles
-    __shared__ RowInfo<BM> ri;
+    __shared__ RowInfo<BM, PRUNED> ri;
     __shared__ int any;
     __shared__ float rv0[BM], rv1[BM], rv2[BM];   // fwd: blank, label logit; bwd: lse, dpx, dpy
     __shared__ float red_m[2][BM], red_s[2][BM];
@@ -244,7 +288,7 @@ __device__ __forceinline__ void logits_tile(const Geo& g, const bf16* __restrict
     const int gq = lane >> 2, cq = lane & 3;
     const float NINF = -INFINITY;
 
-    const bool live = load_rows<BM>(g, r0, ri, &any);
+    const bool live = load_rows<BM, PRUNED>(g, w, r0, ri, &any);
     if (tid < BM) {
         const int f = ri.flag[tid];
         if (!BWD) {
@@ -253,14 +297,16 @@ __device__ __forceinline__ void logits_tile(const Geo& g, const bf16* __restrict
         } else {
             rv0[tid] = (f & 1) ? lse[ri.cell[tid]] : 0.f;
             rv1[tid] = (f & 2) ? dpx[ri.pxi[tid]] : 0.f;
-            rv2[tid] = (f & 1) ? dpy[ri.cell[tid]] : 0.f;
+            rv2[tid] = (f & 1) ? dpy[ri.py(tid)] : 0.f;
         }
     }
     if (!live) {   // every row padding: -inf factors, or zero dlogits
         if (!BWD) {
             if (tid < BM && r0 + tid < g.m) {
-                py[ri.cell[tid]] = NINF;
-                if (ri.pxi[tid] >= 0) px[ri.pxi[tid]] = NINF;
+                if (!PRUNED) {
+                    py[ri.cell[tid]] = NINF;
+                    if (ri.pxi[tid] >= 0) px[ri.pxi[tid]] = NINF;
+                }
                 lse[ri.cell[tid]] = 0.f;
             }
         } else {
@@ -398,48 +444,53 @@ __device__ __forceinline__ void logits_tile(const Geo& g, const bf16* __restrict
                 const float s = red_s[0][tid] * expf(m0 - m) + red_s[1][tid] * expf(m1 - m);
                 const float L = m + logf(s);
                 lse[c] = L;
-                py[c] = rv0[tid] - L;
+                py[ri.py(tid)] = rv0[tid] - L;
                 if (p >= 0) px[p] = (f & 2) ? rv1[tid] - L : NINF;
             } else {
                 lse[c] = 0.f;
-                py[c] = NINF;
-                if (p >= 0) px[p] = NINF;
+                if (!PRUNED) {
+                    py[c] = NINF;
+                    if (p >= 0) px[p] = NINF;
+                }
             }
         }
     }
 }
 
-template <int BM>
+template <int BM, bool PRUNED>
 __global__ void __launch_bounds__(BM * 2) joiner_lse_kernel(Geo g, const bf16* __restrict__ h,
                                                             const bf16* __restrict__ W,
                                                             const bf16* __restrict__ bias, float* __restrict__ lse,
-                                                            float* __restrict__ px, float* __restrict__ py) {
-    logits_tile<false, BM>(g, h, W, bias, lse, px, py, nullptr, nullptr, nullptr);
+                                                            float* __restrict__ px, float* __restrict__ py,
+                                                            Window w) {
+    logits_tile<false, BM, PRUNED>(g, h, W, bias, lse, px, py, nullptr, nullptr, nullptr, w);
 }
 
-template <int BM>
+template <int BM, bool PRUNED>
 __global__ void __launch_bounds__(BM * 2) joiner_dlogits_kernel(Geo g, const bf16* __restrict__ h,
                                                                  const bf16* __restrict__ W,
                                                                  const bf16* __restrict__ bias,
                                                                  const float* __restrict__ lse,
                                                                  const float* __restrict__ dpx,
                                                                  const float* __restrict__ dpy,
-                                                                 bf16* __restrict__ dlog) {
-    logits_tile<true, BM>(g, h, W, bias, const_cast<float*>(lse), nullptr, nullptr, dpx, dpy, dlog);
+                                                                 bf16* __restrict__ dlog, Window w) {
+    logits_tile<true, BM, PRUNED>(g, h, W, bias, const_cast<float*>(lse), nullptr, nullptr, dpx, dpy, dlog, w);
 }
 
 // ds[r, n] = (dlogits[r, :] W[:, n]) act'(h[r, n]) for a 64 x 64 tile (rows r, hidden units n); W is MN-major here.
 // Tiles whose rows are all padding write nothing: the reduction reads valid rows only.
+template <bool PRUNED>
 __global__ void __launch_bounds__(THREADS) joiner_ds_kernel(Geo g, int act, const bf16* __restrict__ dlog,
                                                             const bf16* __restrict__ W,
-                                                            const bf16* __restrict__ h, float* __restrict__ ds) {
+                                                            const bf16* __restrict__ h, float* __restrict__ ds,
+                                                            Window w) {
     extern __shared__ __align__(128) unsigned char smem_raw[];   // PAIR_STAGES A tiles, then as many B tiles
     bf16* sm = reinterpret_cast<bf16*>(smem_raw);
-    __shared__ RowInfo<TILE> ri;
+    __shared__ RowInfo<TILE, PRUNED> ri;
     __shared__ int any;
     const int r0 = blockIdx.x * TILE, n0 = blockIdx.y * TILE;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp >> 1, wn = warp & 1;
-    if (!load_rows<TILE>(g, r0, ri, &any)) return;
+    if (!load_rows<TILE, PRUNED>(g, w, r0, ri, &any)) return;
     bf16* As = sm;
     bf16* Bs = sm + PAIR_STAGES * TILE_ELEMS;
     const int total = g.Vp / TILE;
@@ -490,9 +541,58 @@ __global__ void __launch_bounds__(THREADS) joiner_ds_kernel(Geo g, int act, cons
 }
 
 // denc[b, t] += sum over the chunk's valid cells (b, u, t) of ds, in u order; dpred[b, u] += the same over t, in t
-// order.  One thread per output element: deterministic, no atomics.
+// order.  One thread per output element: deterministic, no atomics.  PRUNED: denc[b, t] sums the chunk's valid rows
+// (b, r, t) in r order; dpred[b, u] sums, in t order over the chunk's frames of b, the valid row r = u - ranges[b,t]
+// where 0 <= r < R.
+template <bool PRUNED>
 __global__ void __launch_bounds__(256) joiner_reduce_kernel(Geo g, const float* __restrict__ ds,
-                                                            float* __restrict__ denc, float* __restrict__ dpred) {
+                                                            float* __restrict__ denc, float* __restrict__ dpred,
+                                                            Window w) {
+    if constexpr (PRUNED) {
+        const int RT = w.R * g.T;                                              // rows per utterance
+        const int b_lo = g.c0 / RT, b_hi = (g.c0 + g.m - 1) / RT;
+        const long long n_pred = (long long)(b_hi - b_lo + 1) * g.U * g.H;
+        const long long n_enc = (long long)(b_hi - b_lo + 1) * g.T * g.H;
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_pred + n_enc;
+             i += (long long)gridDim.x * blockDim.x) {
+            const bool is_pred = i < n_pred;
+            const long long j = is_pred ? i : i - n_pred;
+            const int k = (int)(j % g.H), q = (int)(j / g.H);
+            const int b = b_lo + (is_pred ? q / g.U : q / g.T);
+            const int Tb = clampi(g.xlen[b], 1, g.T), Sb = clampi(g.ylen[b], 0, g.S);
+            const int* rb = w.ranges + (size_t)b * g.T;
+            const int lo = max(g.c0 - b * RT, 0), hi = min(g.c0 + g.m - b * RT, RT);   // b's rows in the chunk
+            float s = 0.f;
+            bool hit = false;
+            if (is_pred) {
+                const int u = q % g.U;
+                if (u > Sb) continue;
+                int t_lo = 0, t_hi = Tb;   // the chunk's frames of b, when its rows of b do not wrap a frame
+                if (hi - lo < g.T && lo % g.T <= (hi - 1) % g.T) t_lo = lo % g.T, t_hi = min((hi - 1) % g.T + 1, Tb);
+                for (int t = t_lo; t < t_hi; ++t) {
+                    const long long r = (long long)u - rb[t];
+                    if (r < 0 || r >= w.R) continue;
+                    const int row = (int)r * g.T + t;
+                    if (row < lo || row >= hi) continue;
+                    s += ds[(size_t)(b * RT + row - g.c0) * g.H + k];
+                    hit = true;
+                }
+                if (hit) dpred[((size_t)b * g.U + u) * g.H + k] += s;
+            } else {
+                const int t = q % g.T;
+                if (t >= Tb) continue;
+                for (int r = 0; r < w.R; ++r) {
+                    const long long u = (long long)rb[t] + r;
+                    const int row = r * g.T + t;
+                    if (u < 0 || u > Sb || row < lo || row >= hi) continue;
+                    s += ds[(size_t)(b * RT + row - g.c0) * g.H + k];
+                    hit = true;
+                }
+                if (hit) denc[((size_t)b * g.T + t) * g.H + k] += s;
+            }
+        }
+        return;
+    }
     const int bu_lo = g.c0 / g.T, bu_hi = (g.c0 + g.m - 1) / g.T;        // (b, u) rows the chunk touches
     const int b_lo = bu_lo / g.U, b_hi = bu_hi / g.U;
     const long long n_pred = (long long)(bu_hi - bu_lo + 1) * g.H;
@@ -608,6 +708,18 @@ __global__ void __launch_bounds__(256) joiner_round_kernel(Geo g, int slabs, con
         } else {
             gp[i - nw - nb - ne] = __float2bfloat16_rn(dpred[i - nw - nb - ne]);
         }
+    }
+}
+
+// px and py of a pruned forward set to -inf before the chunk loop writes the valid rows' cells.
+__global__ void __launch_bounds__(256) joiner_fill_kernel(float* __restrict__ px, long long npx,
+                                                          float* __restrict__ py, long long npy) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npx + npy;
+         i += (long long)gridDim.x * blockDim.x) {
+        if (i < npx)
+            px[i] = -INFINITY;
+        else
+            py[i - npx] = -INFINITY;
     }
 }
 

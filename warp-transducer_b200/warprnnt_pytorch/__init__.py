@@ -145,6 +145,8 @@ __all__ += ['rnnt_forced_align', 'pruned_rnnt_forced_align']
 from .lattice import RNNTLatticeLoss, rnnt_lattice_forced_align, rnnt_lattice_loss  # noqa: E402
 
 __all__ += ['rnnt_lattice_loss', 'RNNTLatticeLoss', 'rnnt_lattice_forced_align']
-from .joiner import JoinerRNNTLoss, joiner_log_probs, joiner_rnnt_loss  # noqa: E402
+from .joiner import (JoinerRNNTLoss, PrunedJoinerRNNTLoss, joiner_log_probs, joiner_rnnt_loss,  # noqa: E402
+                     pruned_joiner_log_probs, pruned_joiner_rnnt_loss)
 
-__all__ += ['joiner_log_probs', 'joiner_rnnt_loss', 'JoinerRNNTLoss']
+__all__ += ['joiner_log_probs', 'joiner_rnnt_loss', 'JoinerRNNTLoss', 'pruned_joiner_log_probs',
+            'pruned_joiner_rnnt_loss', 'PrunedJoinerRNNTLoss']

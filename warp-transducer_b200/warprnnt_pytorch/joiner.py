@@ -13,6 +13,12 @@ backward runs the contraction in reverse, so neither the logits nor their gradie
 
 enc, pred, weight [V, H] (nn.Linear's layout) and bias [V] (or None) are bf16 CUDA tensors; pass a joiner's fp32
 master weights as ``weight.to(torch.bfloat16)`` and autograd carries the gradient back to them.
+
+The pruned step of pruned RNN-T (DESIGN.md §15) runs the same joiner on the windows of the pruning ranges only,
+without the [N, T, R, V] logits of ``prune_joint_inputs`` -> joiner -> ``pruned_rnnt_loss``:
+
+    simple, ranges = add_joint_rnnt_loss_with_ranges(am_proj, lm_proj, labels, act_lens, label_lens, s_range=5)
+    pruned = pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, 5)
 """
 import ctypes as C
 
@@ -35,6 +41,15 @@ _lib.rnnt_b200_joiner_backward.restype = C.c_int
 _lib.rnnt_b200_joiner_backward.argtypes = [C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
                                            _P, _P, _P, _P, _P, _P, _P, warp_rnnt.rnntOptions]
 _lib.rnnt_b200_joiner_last_launch_count.restype = C.c_int
+_lib.rnnt_b200_pruned_joiner_workspace_size.restype = C.c_int
+_lib.rnnt_b200_pruned_joiner_workspace_size.argtypes = [C.c_int] * 7 + [C.POINTER(C.c_size_t)]
+_lib.rnnt_b200_pruned_joiner_forward.restype = C.c_int
+_lib.rnnt_b200_pruned_joiner_forward.argtypes = [C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int,
+                                                 C.c_int, C.c_int, _P, _P, _P, warp_rnnt.rnntOptions]
+_lib.rnnt_b200_pruned_joiner_backward.restype = C.c_int
+_lib.rnnt_b200_pruned_joiner_backward.argtypes = [C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int,
+                                                  C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P,
+                                                  warp_rnnt.rnntOptions]
 
 RNNT_B200_ACT_TANH, RNNT_B200_ACT_RELU = 0, 1
 _ACTIVATIONS = {'tanh': RNNT_B200_ACT_TANH, 'relu': RNNT_B200_ACT_RELU}
@@ -55,13 +70,20 @@ def _chunk(chunk_cells):
     return chunk_cells
 
 
-def workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells=None):
-    """Bytes of the joiner's workspace (include/rnnt.h rnnt_b200_joiner_workspace_size)."""
+def workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells=None, s_range=None):
+    """Bytes of the joiner's workspace (include/rnnt.h rnnt_b200_joiner_workspace_size), or with s_range of the
+    pruned joiner's (rnnt_b200_pruned_joiner_workspace_size)."""
     n = C.c_size_t(0)
-    st = _lib.rnnt_b200_joiner_workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, _chunk(chunk_cells),
-                                              C.byref(n))
+    if s_range is None:
+        name = "rnnt_b200_joiner_workspace_size"
+        st = _lib.rnnt_b200_joiner_workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, _chunk(chunk_cells),
+                                                  C.byref(n))
+    else:
+        name = "rnnt_b200_pruned_joiner_workspace_size"
+        st = _lib.rnnt_b200_pruned_joiner_workspace_size(maxT, maxU, s_range, minibatch, hidden, alphabet_size,
+                                                         _chunk(chunk_cells), C.byref(n))
     if st != warp_rnnt.RNNT_STATUS_SUCCESS:
-        raise ValueError("rnnt_b200_joiner_workspace_size: " + warp_rnnt.status_string(st))
+        raise ValueError(name + ": " + warp_rnnt.status_string(st))
     return n.value
 
 
@@ -70,10 +92,28 @@ def last_launch_count():
     return _lib.rnnt_b200_joiner_last_launch_count()
 
 
-def _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells):
+def _check_window(ranges, s_range, N, T):
+    """pruned_rnnt_loss's rules for ranges (int32 [N, T], contiguous) and a positive int s_range, N T R < 2^31.  A
+    pruned call always has its window: ranges=None is a TypeError, never the dense joiner."""
+    if not isinstance(ranges, torch.Tensor):
+        raise TypeError("ranges must be an int32 tensor [N, T], got %s" % type(ranges).__name__)
+    if isinstance(s_range, bool) or not isinstance(s_range, int) or s_range < 1:
+        raise ValueError("s_range must be a positive int, got %r" % (s_range,))
+    check_type(ranges, torch.int32, "ranges")
+    check_contiguous(ranges, "ranges")
+    check_dim(ranges, 2, "ranges")
+    if tuple(ranges.shape) != (N, T):
+        raise ValueError("ranges must be [N, T] = [%d, %d], got %s" % (N, T, tuple(ranges.shape)))
+    if N * T * s_range >= 2 ** 31:
+        raise ValueError("N * T * s_range must be below 2^31, got %d" % (N * T * s_range))
+
+
+def _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells,
+                  window=None):
     """rnnt_loss's rules and exception types: ValueError for an option, a rank, a shape, an extent or a
-    non-contiguous tensor, TypeError for a dtype, RuntimeError for a CPU tensor or a second device.  Returns the
-    deferred T == max(act_lens), S == max(label_lens) check."""
+    non-contiguous tensor, TypeError for a dtype, RuntimeError for a CPU tensor or a second device.  With a window
+    (ranges, s_range), a pruned call, pruned_rnnt_loss's rules for it too.  Returns the deferred T == max(act_lens),
+    S == max(label_lens) check."""
     activation_code(activation)
     _chunk(chunk_cells)
     for name, t in (("enc", enc), ("pred", pred), ("weight", weight), ("bias", bias)):
@@ -115,6 +155,9 @@ def _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, 
     if N * T * U >= 2 ** 31:
         raise ValueError("N * T * U must be below 2^31, got %d" % (N * T * U))
     tensors = dict(pred=pred, weight=weight, bias=bias, labels=labels, act_lens=act_lens, label_lens=label_lens)
+    if window is not None:
+        _check_window(*window, N, T)
+        tensors["ranges"] = window[0]
     if not all(t.is_cuda for t in [enc] + [t for t in tensors.values() if t is not None]):
         raise RuntimeError("warprnnt_pytorch (H100 build) runs on CUDA tensors only; there is no CPU fallback")
     warp_rnnt.require_same_device(enc, **tensors)
@@ -135,66 +178,81 @@ def _ptr(t):
     return t.data_ptr() if t is not None and t.numel() > 0 else None
 
 
+def _inputs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range):
+    """The entry's name and its leading arguments (the window follows the lengths on the pruned entries).  Either
+    of ranges and s_range makes the call pruned, and a pruned call needs both."""
+    head = [enc.data_ptr(), pred.data_ptr(), weight.data_ptr(), _ptr(bias), _ptr(labels), label_lens.data_ptr(),
+            act_lens.data_ptr()]
+    if ranges is None and s_range is None:
+        return "rnnt_b200_joiner", head
+    if ranges is None or s_range is None:
+        raise ValueError("a pruned joiner call needs both ranges and s_range")
+    return "rnnt_b200_pruned_joiner", head + [ranges.data_ptr(), s_range]
+
+
 def gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px, py, blank, activation,
-                       chunk_cells=None, workspace=None):
+                       chunk_cells=None, workspace=None, ranges=None, s_range=None):
     """px [N, S, T] and py [N, S+1, T] (float32, every element written) from the joiner's inputs, checked by the
-    caller (include/rnnt.h rnnt_b200_joiner_forward).  Returns the workspace, which the backward reads."""
+    caller (include/rnnt.h rnnt_b200_joiner_forward; with ranges and s_range, rnnt_b200_pruned_joiner_forward).
+    Returns the workspace, which the backward reads."""
     N, T, H = enc.shape
     U, V = pred.shape[1], weight.shape[0]
+    name, head = _inputs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range)
     with torch.cuda.device(enc.device):
-        need = workspace_size(T, U, N, H, V, chunk_cells)
+        need = workspace_size(T, U, N, H, V, chunk_cells, s_range)
         if workspace is None or workspace.numel() < need:
             workspace = torch.empty(need, dtype=torch.uint8, device=enc.device)
-        st = _lib.rnnt_b200_joiner_forward(activation_code(activation), enc.data_ptr(), pred.data_ptr(),
-                                           weight.data_ptr(), _ptr(bias), _ptr(labels), label_lens.data_ptr(),
-                                           act_lens.data_ptr(), H, V, N, _chunk(chunk_cells), _ptr(px),
-                                           py.data_ptr(), workspace.data_ptr(), _options(enc, U, blank))
+        st = getattr(_lib, name + "_forward")(activation_code(activation), *head, H, V, N, _chunk(chunk_cells),
+                                              _ptr(px), py.data_ptr(), workspace.data_ptr(), _options(enc, U, blank))
     if st != warp_rnnt.RNNT_STATUS_SUCCESS:
-        raise RuntimeError("rnnt_b200_joiner_forward failed: " + warp_rnnt.status_string(st))
+        raise RuntimeError(name + "_forward failed: " + warp_rnnt.status_string(st))
     return workspace
 
 
 def gpu_joiner_backward(enc, pred, weight, bias, labels, act_lens, label_lens, dpx, dpy, grad_enc, grad_pred,
-                        grad_weight, grad_bias, blank, activation, chunk_cells, workspace):
+                        grad_weight, grad_bias, blank, activation, chunk_cells, workspace, ranges=None,
+                        s_range=None):
     """The four bf16 gradients from dpx, dpy (float32, shaped as px, py) and the workspace of gpu_joiner_forward
-    with the same arguments (include/rnnt.h rnnt_b200_joiner_backward)."""
+    with the same arguments (include/rnnt.h rnnt_b200_joiner_backward / rnnt_b200_pruned_joiner_backward)."""
     N, T, H = enc.shape
     U, V = pred.shape[1], weight.shape[0]
+    name, head = _inputs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range)
     with torch.cuda.device(enc.device):
-        st = _lib.rnnt_b200_joiner_backward(activation_code(activation), enc.data_ptr(), pred.data_ptr(),
-                                            weight.data_ptr(), _ptr(bias), _ptr(labels), label_lens.data_ptr(),
-                                            act_lens.data_ptr(), H, V, N, _chunk(chunk_cells), _ptr(dpx),
-                                            dpy.data_ptr(), grad_enc.data_ptr(), grad_pred.data_ptr(),
-                                            grad_weight.data_ptr(), _ptr(grad_bias), workspace.data_ptr(),
-                                            _options(enc, U, blank))
+        st = getattr(_lib, name + "_backward")(activation_code(activation), *head, H, V, N, _chunk(chunk_cells),
+                                               _ptr(dpx), dpy.data_ptr(), grad_enc.data_ptr(), grad_pred.data_ptr(),
+                                               grad_weight.data_ptr(), _ptr(grad_bias), workspace.data_ptr(),
+                                               _options(enc, U, blank))
     if st != warp_rnnt.RNNT_STATUS_SUCCESS:
-        raise RuntimeError("rnnt_b200_joiner_backward failed: " + warp_rnnt.status_string(st))
+        raise RuntimeError(name + "_backward failed: " + warp_rnnt.status_string(st))
 
 
 class _JoinerLogProbs(Function):
-    """forward: 2 launches per chunk, px / py and the per-cell lse.  backward: 5 launches per chunk and 1 more,
-    from the lse the forward left in the workspace."""
+    """The dense joiner (window None), or with a window (ranges, s_range) the pruned one.  forward: 2 launches per
+    chunk (the pruned call 1 more, the -inf fill), px / py and the per-row lse.  backward: 5 launches per chunk and 1
+    more, from the lse the forward left in the workspace."""
 
     @staticmethod
-    def forward(ctx, enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells):
+    def forward(ctx, enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells,
+                window=None):
         length_check = _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
-                                     chunk_cells)
+                                     chunk_cells, window)
+        ranges, s_range = window if window is not None else (None, None)
         N, T, _ = enc.shape
         S = pred.shape[1] - 1
         px = torch.empty((N, S, T), dtype=torch.float32, device=enc.device)
         py = torch.empty((N, S + 1, T), dtype=torch.float32, device=enc.device)
         ws = gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px, py, blank, activation,
-                                chunk_cells)
+                                chunk_cells, ranges=ranges, s_range=s_range)
         length_check.finish()
-        ctx.save_for_backward(enc, pred, weight, bias, labels, act_lens, label_lens)
+        ctx.save_for_backward(enc, pred, weight, bias, labels, act_lens, label_lens, ranges)
         ctx.workspace = ws
-        ctx.args = (blank, activation, chunk_cells)
+        ctx.args = (blank, activation, chunk_cells, s_range)
         return px, py
 
     @staticmethod
     def backward(ctx, dpx, dpy):
-        enc, pred, weight, bias, labels, act_lens, label_lens = ctx.saved_tensors
-        blank, activation, chunk_cells = ctx.args
+        enc, pred, weight, bias, labels, act_lens, label_lens, ranges = ctx.saved_tensors
+        blank, activation, chunk_cells, s_range = ctx.args
         N, T, _ = enc.shape
         S = pred.shape[1] - 1
         dpx = (torch.zeros((N, S, T), dtype=torch.float32, device=enc.device) if dpx is None
@@ -204,10 +262,10 @@ class _JoinerLogProbs(Function):
         grad_enc, grad_pred, grad_weight = torch.empty_like(enc), torch.empty_like(pred), torch.empty_like(weight)
         grad_bias = torch.empty_like(bias) if bias is not None else None
         gpu_joiner_backward(enc, pred, weight, bias, labels, act_lens, label_lens, dpx, dpy, grad_enc, grad_pred,
-                            grad_weight, grad_bias, blank, activation, chunk_cells, ctx.workspace)
+                            grad_weight, grad_bias, blank, activation, chunk_cells, ctx.workspace, ranges, s_range)
         need = ctx.needs_input_grad
         return (grad_enc if need[0] else None, grad_pred if need[1] else None, grad_weight if need[2] else None,
-                grad_bias if bias is not None and need[3] else None, None, None, None, None, None, None)
+                grad_bias if bias is not None and need[3] else None, None, None, None, None, None, None, None)
 
 
 def joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blank=0, *, activation='tanh',
@@ -231,6 +289,21 @@ def joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blan
                                  chunk_cells)
 
 
+def pruned_joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range, blank=0, *,
+                            activation='tanh', chunk_cells=None):
+    """joiner_log_probs on the pruned lattice of pruned_rnnt_loss, without the [N, T, R, V] logits (DESIGN.md §15).
+
+    ranges [N, T] int32 (contiguous, on the inputs' device) and s_range = R, a positive int: row (b, t, r), r < R,
+    stands for cell (t, ranges[b, t] + r), and is padding unless t < T_b and 0 <= ranges[b, t] + r <= S_b (any int32
+    start is allowed, and R > U).  Returns px [N, U-1, T] and py [N, U, T] as joiner_log_probs does: its values on
+    the cells a valid row covers, -inf everywhere else; dpx / dpy are read only on those cells.  The other arguments
+    and the gradients are joiner_log_probs's; chunk_cells counts rows (b, t, r).  With s_range = U and ranges == 0
+    both the factors and the gradients are bitwise joiner_log_probs's.  The alignment of the pruned lattice is
+    rnnt_lattice_forced_align(*pruned_joiner_log_probs(...), act_lens, label_lens)."""
+    return _JoinerLogProbs.apply(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
+                                 chunk_cells, (ranges, s_range))
+
+
 def _delay(px, act_lens, delay_penalty):
     """px + delay_penalty ((T_b - 1) / 2 - t): rnnt_loss's delay-penalised label factors."""
     T = px.shape[2]
@@ -247,11 +320,32 @@ def joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, blan
         rnnt_lattice_loss(px + delay_penalty ((T_b - 1)/2 - t), py, act_lens, label_lens, reduction, rnnt_type)
 
     on (px, py) = joiner_log_probs(...).  reduction, rnnt_type and delay_penalty are rnnt_loss's."""
+    return _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reduction, activation, rnnt_type,
+                 delay_penalty)
+
+
+def pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range, blank=0,
+                            reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+    """Pruned RNN-T loss of the joiner  logits = weight act(enc[b,t] + pred[b,u]) + bias  on the windows
+    (ranges, s_range) of add_joint_rnnt_loss_with_ranges, without the [N, T, R, V] logits or their gradient: what
+    prune_joint_inputs -> joiner -> pruned_rnnt_loss computes, as
+
+        rnnt_lattice_loss(px + delay_penalty ((T_b - 1)/2 - t), py, act_lens, label_lens, reduction, rnnt_type)
+
+    on (px, py) = pruned_joiner_log_probs(...).  An utterance whose windows leave no path costs +inf with zero
+    gradients.  reduction, rnnt_type and delay_penalty are pruned_rnnt_loss's."""
+    return _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reduction, activation, rnnt_type,
+                 delay_penalty, (ranges, s_range))
+
+
+def _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reduction, activation, rnnt_type,
+          delay_penalty, window=None):
     warp_rnnt.rnnt_type_code(rnnt_type)
     warp_rnnt.lattice_options(delay_penalty)
     if reduction not in ('none', 'sum', 'mean'):
         raise ValueError("reduction must be 'none', 'sum' or 'mean'")
-    px, py = joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation=activation)
+    px, py = _JoinerLogProbs.apply(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, None,
+                                   window)
     if delay_penalty:
         px = _delay(px, act_lens, float(delay_penalty))
     return rnnt_lattice_loss(px, py, act_lens, label_lens, reduction, rnnt_type=rnnt_type)
@@ -275,3 +369,24 @@ class JoinerRNNTLoss(Module):
         return joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, self.blank, self.reduction,
                                 activation=self.activation, rnnt_type=self.rnnt_type,
                                 delay_penalty=self.delay_penalty)
+
+
+class PrunedJoinerRNNTLoss(Module):
+    """Module form of pruned_joiner_rnnt_loss: PrunedJoinerRNNTLoss(blank=0, reduction='mean', *, activation='tanh',
+    rnnt_type='regular', delay_penalty=0.0); forward(enc, pred, weight, bias, labels, act_lens, label_lens, ranges,
+    s_range)."""
+
+    def __init__(self, blank=0, reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+        super().__init__()
+        activation_code(activation)
+        warp_rnnt.rnnt_type_code(rnnt_type)
+        warp_rnnt.lattice_options(delay_penalty)
+        if reduction not in ('none', 'sum', 'mean'):
+            raise ValueError("reduction must be 'none', 'sum' or 'mean'")
+        self.blank, self.reduction = blank, reduction
+        self.activation, self.rnnt_type, self.delay_penalty = activation, rnnt_type, delay_penalty
+
+    def forward(self, enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range):
+        return pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range,
+                                       self.blank, self.reduction, activation=self.activation,
+                                       rnnt_type=self.rnnt_type, delay_penalty=self.delay_penalty)

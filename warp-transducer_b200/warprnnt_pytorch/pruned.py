@@ -11,6 +11,10 @@ A training step with a real (nonlinear) joiner:
 
 The pruned loss reads R logits per frame instead of U: row (b, t, s) of `logits` is lattice cell
 (t, ranges[b, t] + s).  Cells no row covers cannot be visited; rows outside the utterance get a zero gradient.
+
+For icefall's joiner, logits = W act(enc + pred) + bias, the middle three lines are one call that never forms the
+[N, T, R, V] logits: pruned_joiner_rnnt_loss(enc, pred, W, bias, labels, act_lens, label_lens, ranges, 5)
+(joiner.py, DESIGN.md §15).
 """
 import ctypes as C
 
