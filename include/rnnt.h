@@ -716,6 +716,57 @@ rnntStatus_t rnnt_b200_pruned_joiner_backward(int activation, const void* enc, c
                                               int alphabet_size, int minibatch, int chunk_cells, const float* dpx,
                                               const float* dpy, void* grad_enc, void* grad_pred, void* grad_weight,
                                               void* grad_bias, void* workspace, struct rnntOptions options);
+
+/* Dropout on the joiner's hidden activation (DESIGN.md §16): NeMo's RNNTJoint, Sequential(act, Dropout(p), Linear),
+ * for the fused and pruned fused joiners.  Passed BY VALUE to the *_drop entries below, which take the arguments of
+ * the entry of the same name and this before the workspace.
+ *   p      dropout probability, 0 <= p < 1.
+ *   seed   device pointer to a 64-bit seed, 8-byte aligned, read on the device (no host synchronisation; graph
+ *          capture records the pointer, so a replay uses whatever seed it then holds).  May be NULL when p == 0.
+ * Mask: element k of cell (b, t, u) is dropped iff x < thr, with x = word (k & 3) of
+ *   curand_Philox4x32_10(ctr = (k >> 2, (b maxU + u) maxT + t, 0, 0), key = (lo32(seed), hi32(seed)))
+ * and thr = floor((double) p 2^32).  It is a pure function of the seed and the element: the same for any chunk_cells,
+ * dense or pruned, forward or backward, so nothing is stored.  It depends on the padded extents maxT and maxU, as
+ * eager dropout on an [N, maxT, maxU, hidden] tensor does.  A pruned row uses the mask of the cell it stands for.
+ * forward: the logits GEMM operand is h~ = keep ? round_bf16(h scale) : 0, scale = (float)(1 / (1 - (double) p)),
+ *   with h the fused joiner's rounded h; px, py follow from h~.  The bias column is never dropped.
+ * backward: dlogit as without dropout; grad_weight = sum dlogit (x) h~; ds = (dlogit weight) keep scale act'(s), act'
+ *   as without dropout (tanh: 1 - h^2 from the undropped rounded h).  The backward must get the forward's p and seed.
+ * Workspace sizes, launches and every other rule are those of the entry of the same name; p == 0 runs its kernels
+ * and gives its results bitwise.  NaN p, p < 0, p >= 1, a NULL seed with p > 0 and a misaligned seed are
+ * RNNT_STATUS_INVALID_VALUE before any device access. */
+struct rnntJoinerDropout {
+    float p;
+    const unsigned long long* seed;
+};
+rnntStatus_t rnnt_b200_joiner_forward_drop(int activation, const void* enc, const void* pred, const void* weight,
+                                           const void* bias, const int* flat_labels, const int* label_lengths,
+                                           const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                           int chunk_cells, float* px, float* py, struct rnntJoinerDropout dropout,
+                                           void* workspace, struct rnntOptions options);
+rnntStatus_t rnnt_b200_joiner_backward_drop(int activation, const void* enc, const void* pred, const void* weight,
+                                            const void* bias, const int* flat_labels, const int* label_lengths,
+                                            const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                            int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
+                                            void* grad_pred, void* grad_weight, void* grad_bias,
+                                            struct rnntJoinerDropout dropout, void* workspace,
+                                            struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_joiner_forward_drop(int activation, const void* enc, const void* pred,
+                                                  const void* weight, const void* bias, const int* flat_labels,
+                                                  const int* label_lengths, const int* input_lengths,
+                                                  const int* ranges, int s_range, int hidden, int alphabet_size,
+                                                  int minibatch, int chunk_cells, float* px, float* py,
+                                                  struct rnntJoinerDropout dropout, void* workspace,
+                                                  struct rnntOptions options);
+rnntStatus_t rnnt_b200_pruned_joiner_backward_drop(int activation, const void* enc, const void* pred,
+                                                   const void* weight, const void* bias, const int* flat_labels,
+                                                   const int* label_lengths, const int* input_lengths,
+                                                   const int* ranges, int s_range, int hidden, int alphabet_size,
+                                                   int minibatch, int chunk_cells, const float* dpx,
+                                                   const float* dpy, void* grad_enc, void* grad_pred,
+                                                   void* grad_weight, void* grad_bias,
+                                                   struct rnntJoinerDropout dropout, void* workspace,
+                                                   struct rnntOptions options);
 /* Kernels (memsets not counted) the last fused or pruned joiner call on this thread launched. */
 int rnnt_b200_joiner_last_launch_count(void);
 

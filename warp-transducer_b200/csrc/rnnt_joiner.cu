@@ -1,10 +1,12 @@
 // C-ABI of the fused joiner (include/rnnt.h, DESIGN.md §14) and of the pruned fused joiner (§15): workspace sizing,
-// argument rules and the chunk loop, shared by both; the pruned calls run the same loop over N T R window rows.
+// argument rules and the chunk loop, shared by both; the pruned calls run the same loop over N T R window rows.  The
+// _drop entries (§16) are the same calls with dropout on h; the entries without it are them with p = 0.
 // A translation unit of its own, so the kernels of rnnt_entry.cu compile exactly as they did without it.
 #include <cuda_runtime.h>
 
 #include <atomic>
 #include <climits>
+#include <cmath>
 #include <cstdint>
 
 #include "../../include/rnnt.h"
@@ -117,7 +119,8 @@ bool allow_smem(cudaFuncAttribute attr, int big, int small) {
            cudaFuncSetAttribute(joiner_dlogits_kernel<128, PRUNED>, attr, big) == cudaSuccess &&
            cudaFuncSetAttribute(joiner_lse_kernel<64, PRUNED>, attr, small) == cudaSuccess &&
            cudaFuncSetAttribute(joiner_dlogits_kernel<64, PRUNED>, attr, small) == cudaSuccess &&
-           cudaFuncSetAttribute(joiner_ds_kernel<PRUNED>, attr, (int)kPairSmem) == cudaSuccess;
+           cudaFuncSetAttribute(joiner_ds_kernel<PRUNED>, attr, (int)kPairSmem) == cudaSuccess &&
+           cudaFuncSetAttribute(joiner_ds_kernel<PRUNED, true>, attr, (int)kPairSmem) == cudaSuccess;
 }
 
 // The dynamic shared-memory opt-in of every kernel, dense and pruned, for the largest call, once per device: after
@@ -147,8 +150,12 @@ rnntStatus_t launched() {
 
 template <bool PRUNED>
 void launch_h(const Geo& g, int act, const bf16* enc, const bf16* pred, bf16* h, int rows, cudaStream_t s,
-              const Window& w) {
-    joiner_h_kernel<PRUNED><<<blocks((long long)rows * (g.Hp / 8), 256), 256, 0, s>>>(g, act, enc, pred, h, rows, w);
+              const Window& w, const Drop& d) {
+    const int nb = blocks((long long)rows * (g.Hp / 8), 256);
+    if (d.seed)
+        joiner_h_kernel<PRUNED, true><<<nb, 256, 0, s>>>(g, act, enc, pred, h, rows, w, d);
+    else
+        joiner_h_kernel<PRUNED><<<nb, 256, 0, s>>>(g, act, enc, pred, h, rows, w);
     ++g_joiner_launches;
 }
 
@@ -157,7 +164,7 @@ template <bool PRUNED>
 rnntStatus_t forward(int activation, const void* enc, const void* pred, const void* weight, const void* bias,
                      const int* flat_labels, const int* label_lengths, const int* input_lengths, int hidden,
                      int alphabet_size, int minibatch, int chunk_cells, float* px, float* py, void* workspace,
-                     const rnntOptions& options, const Window& w) {
+                     const rnntOptions& options, const Window& w, const Drop& d) {
     const Plan p = plan(options.maxT, options.maxU, minibatch, hidden, alphabet_size, chunk_cells,
                         PRUNED ? w.R : options.maxU);
     char* ws = static_cast<char*>(workspace);
@@ -180,7 +187,7 @@ rnntStatus_t forward(int activation, const void* enc, const void* pred, const vo
         g.m = p.cells - c0 < p.chunk ? p.cells - c0 : p.chunk;
         const int tiles = (g.m + bm - 1) / bm;
         launch_h<PRUNED>(g, activation, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred), h, tiles * bm,
-                         s, w);
+                         s, w, d);
         if (bm == 128)
             joiner_lse_kernel<128, PRUNED><<<tiles, 256, smem, s>>>(g, h, W, B, lse, px, py, w);
         else
@@ -196,7 +203,7 @@ rnntStatus_t backward(int activation, const void* enc, const void* pred, const v
                       const int* flat_labels, const int* label_lengths, const int* input_lengths, int hidden,
                       int alphabet_size, int minibatch, int chunk_cells, const float* dpx, const float* dpy,
                       void* grad_enc, void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
-                      const rnntOptions& options, const Window& w) {
+                      const rnntOptions& options, const Window& w, const Drop& d) {
     const Plan p = plan(options.maxT, options.maxU, minibatch, hidden, alphabet_size, chunk_cells,
                         PRUNED ? w.R : options.maxU);
     char* ws = static_cast<char*>(workspace);
@@ -222,15 +229,19 @@ rnntStatus_t backward(int activation, const void* enc, const void* pred, const v
         g.m = p.cells - c0 < p.chunk ? p.cells - c0 : p.chunk;
         const int ltiles = (g.m + bm - 1) / bm, tiles = (g.m + TILE - 1) / TILE;
         launch_h<PRUNED>(g, activation, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred), h,
-                         ltiles * bm, s, w);
+                         ltiles * bm, s, w, d);
         if (bm == 128)
             joiner_dlogits_kernel<128, PRUNED><<<ltiles, 256, smem, s>>>(g, h, W, static_cast<const bf16*>(bias), lse,
                                                                          dpx, dpy, dlog, w);
         else
             joiner_dlogits_kernel<64, PRUNED><<<ltiles, 128, smem, s>>>(g, h, W, static_cast<const bf16*>(bias), lse,
                                                                         dpx, dpy, dlog, w);
-        joiner_ds_kernel<PRUNED><<<dim3(tiles, (p.H + TILE - 1) / TILE), THREADS, kPairSmem, s>>>(g, activation, dlog,
-                                                                                                  W, h, ds, w);
+        const dim3 ds_grid(tiles, (p.H + TILE - 1) / TILE);
+        if (d.seed)
+            joiner_ds_kernel<PRUNED, true><<<ds_grid, THREADS, kPairSmem, s>>>(
+                g, activation, dlog, W, h, ds, w, d, static_cast<const bf16*>(enc), static_cast<const bf16*>(pred));
+        else
+            joiner_ds_kernel<PRUNED><<<ds_grid, THREADS, kPairSmem, s>>>(g, activation, dlog, W, h, ds, w);
         const int bu_lo = c0 / p.T, bu_hi = (c0 + g.m - 1) / p.T;
         const long long b_n = bu_hi / per_b - bu_lo / per_b + 1;
         // dense: one thread per (b, u) row and per (b, t) of the chunk; pruned: per (b, u) and (b, t) of its b
@@ -249,6 +260,21 @@ rnntStatus_t backward(int activation, const void* enc, const void* pred, const v
     return launched();
 }
 
+// The dropout rules of the _drop entries: 0 <= p < 1 (NaN fails), a seed when p > 0, 8-byte aligned when given.
+bool dropout_ok(const rnntJoinerDropout& o) {
+    if (!(o.p >= 0.f && o.p < 1.f)) return false;
+    if (o.p > 0.f && !o.seed) return false;
+    return (reinterpret_cast<uintptr_t>(o.seed) & 7) == 0;
+}
+
+// The kernels' descriptor: no seed (the DROP = false kernels) when p == 0.
+Drop drop(const rnntJoinerDropout& o) {
+    if (!(o.p > 0.f)) return Drop{nullptr, 0u, 1.f};
+    return Drop{o.seed, (uint32_t)floor((double)o.p * 4294967296.0), (float)(1.0 / (1.0 - (double)o.p))};
+}
+
+const rnntJoinerDropout kNoDropout = {0.f, nullptr};
+
 }  // namespace
 
 extern "C" {
@@ -266,14 +292,9 @@ rnntStatus_t rnnt_b200_joiner_forward(int activation, const void* enc, const voi
                                       const int* input_lengths, int hidden, int alphabet_size, int minibatch,
                                       int chunk_cells, float* px, float* py, void* workspace,
                                       struct rnntOptions options) {
-    g_joiner_launches = 0;
-    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
-                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
-    if (st != RNNT_STATUS_SUCCESS) return st;
-    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
-    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
-    return forward<false>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
-                          alphabet_size, minibatch, chunk_cells, px, py, workspace, options, Window{nullptr, 0});
+    return rnnt_b200_joiner_forward_drop(activation, enc, pred, weight, bias, flat_labels, label_lengths,
+                                         input_lengths, hidden, alphabet_size, minibatch, chunk_cells, px, py,
+                                         kNoDropout, workspace, options);
 }
 
 rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
@@ -282,16 +303,46 @@ rnntStatus_t rnnt_b200_joiner_backward(int activation, const void* enc, const vo
                                        int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
                                        void* grad_pred, void* grad_weight, void* grad_bias, void* workspace,
                                        struct rnntOptions options) {
+    return rnnt_b200_joiner_backward_drop(activation, enc, pred, weight, bias, flat_labels, label_lengths,
+                                          input_lengths, hidden, alphabet_size, minibatch, chunk_cells, dpx, dpy,
+                                          grad_enc, grad_pred, grad_weight, grad_bias, kNoDropout, workspace, options);
+}
+
+rnntStatus_t rnnt_b200_joiner_forward_drop(int activation, const void* enc, const void* pred, const void* weight,
+                                           const void* bias, const int* flat_labels, const int* label_lengths,
+                                           const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                           int chunk_cells, float* px, float* py, struct rnntJoinerDropout dropout,
+                                           void* workspace, struct rnntOptions options) {
     g_joiner_launches = 0;
     rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
                                    hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
     if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!dropout_ok(dropout)) return RNNT_STATUS_INVALID_VALUE;
+    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
+    return forward<false>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
+                          alphabet_size, minibatch, chunk_cells, px, py, workspace, options, Window{nullptr, 0},
+                          drop(dropout));
+}
+
+rnntStatus_t rnnt_b200_joiner_backward_drop(int activation, const void* enc, const void* pred, const void* weight,
+                                            const void* bias, const int* flat_labels, const int* label_lengths,
+                                            const int* input_lengths, int hidden, int alphabet_size, int minibatch,
+                                            int chunk_cells, const float* dpx, const float* dpy, void* grad_enc,
+                                            void* grad_pred, void* grad_weight, void* grad_bias,
+                                            struct rnntJoinerDropout dropout, void* workspace,
+                                            struct rnntOptions options) {
+    g_joiner_launches = 0;
+    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
+                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
+    if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!dropout_ok(dropout)) return RNNT_STATUS_INVALID_VALUE;
     if (!dpy || (!dpx && options.maxU > 1) || !grad_enc || !grad_pred || !grad_weight)
         return RNNT_STATUS_INVALID_VALUE;
     if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
     return backward<false>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
                            alphabet_size, minibatch, chunk_cells, dpx, dpy, grad_enc, grad_pred, grad_weight,
-                           grad_bias, workspace, options, Window{nullptr, 0});
+                           grad_bias, workspace, options, Window{nullptr, 0}, drop(dropout));
 }
 
 rnntStatus_t rnnt_b200_pruned_joiner_workspace_size(int maxT, int maxU, int s_range, int minibatch, int hidden,
@@ -308,15 +359,9 @@ rnntStatus_t rnnt_b200_pruned_joiner_forward(int activation, const void* enc, co
                                              const int* input_lengths, const int* ranges, int s_range, int hidden,
                                              int alphabet_size, int minibatch, int chunk_cells, float* px, float* py,
                                              void* workspace, struct rnntOptions options) {
-    g_joiner_launches = 0;
-    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
-                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
-    if (st != RNNT_STATUS_SUCCESS) return st;
-    if (!ranges || !window_ok(options.maxT, minibatch, s_range)) return RNNT_STATUS_INVALID_VALUE;
-    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
-    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
-    return forward<true>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
-                         alphabet_size, minibatch, chunk_cells, px, py, workspace, options, Window{ranges, s_range});
+    return rnnt_b200_pruned_joiner_forward_drop(activation, enc, pred, weight, bias, flat_labels, label_lengths,
+                                                input_lengths, ranges, s_range, hidden, alphabet_size, minibatch,
+                                                chunk_cells, px, py, kNoDropout, workspace, options);
 }
 
 rnntStatus_t rnnt_b200_pruned_joiner_backward(int activation, const void* enc, const void* pred, const void* weight,
@@ -325,17 +370,53 @@ rnntStatus_t rnnt_b200_pruned_joiner_backward(int activation, const void* enc, c
                                               int alphabet_size, int minibatch, int chunk_cells, const float* dpx,
                                               const float* dpy, void* grad_enc, void* grad_pred, void* grad_weight,
                                               void* grad_bias, void* workspace, struct rnntOptions options) {
+    return rnnt_b200_pruned_joiner_backward_drop(activation, enc, pred, weight, bias, flat_labels, label_lengths,
+                                                 input_lengths, ranges, s_range, hidden, alphabet_size, minibatch,
+                                                 chunk_cells, dpx, dpy, grad_enc, grad_pred, grad_weight, grad_bias,
+                                                 kNoDropout, workspace, options);
+}
+
+rnntStatus_t rnnt_b200_pruned_joiner_forward_drop(int activation, const void* enc, const void* pred,
+                                                  const void* weight, const void* bias, const int* flat_labels,
+                                                  const int* label_lengths, const int* input_lengths,
+                                                  const int* ranges, int s_range, int hidden, int alphabet_size,
+                                                  int minibatch, int chunk_cells, float* px, float* py,
+                                                  struct rnntJoinerDropout dropout, void* workspace,
+                                                  struct rnntOptions options) {
     g_joiner_launches = 0;
     rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
                                    hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
     if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!dropout_ok(dropout)) return RNNT_STATUS_INVALID_VALUE;
+    if (!ranges || !window_ok(options.maxT, minibatch, s_range)) return RNNT_STATUS_INVALID_VALUE;
+    if (!py || (!px && options.maxU > 1)) return RNNT_STATUS_INVALID_VALUE;
+    if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
+    return forward<true>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
+                         alphabet_size, minibatch, chunk_cells, px, py, workspace, options, Window{ranges, s_range},
+                         drop(dropout));
+}
+
+rnntStatus_t rnnt_b200_pruned_joiner_backward_drop(int activation, const void* enc, const void* pred,
+                                                   const void* weight, const void* bias, const int* flat_labels,
+                                                   const int* label_lengths, const int* input_lengths,
+                                                   const int* ranges, int s_range, int hidden, int alphabet_size,
+                                                   int minibatch, int chunk_cells, const float* dpx,
+                                                   const float* dpy, void* grad_enc, void* grad_pred,
+                                                   void* grad_weight, void* grad_bias,
+                                                   struct rnntJoinerDropout dropout, void* workspace,
+                                                   struct rnntOptions options) {
+    g_joiner_launches = 0;
+    rnntStatus_t st = check_common(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths,
+                                   hidden, alphabet_size, minibatch, chunk_cells, workspace, options);
+    if (st != RNNT_STATUS_SUCCESS) return st;
+    if (!dropout_ok(dropout)) return RNNT_STATUS_INVALID_VALUE;
     if (!ranges || !window_ok(options.maxT, minibatch, s_range)) return RNNT_STATUS_INVALID_VALUE;
     if (!dpy || (!dpx && options.maxU > 1) || !grad_enc || !grad_pred || !grad_weight)
         return RNNT_STATUS_INVALID_VALUE;
     if (options.loc != RNNT_GPU) return RNNT_STATUS_EXECUTION_FAILED;
     return backward<true>(activation, enc, pred, weight, bias, flat_labels, label_lengths, input_lengths, hidden,
                           alphabet_size, minibatch, chunk_cells, dpx, dpy, grad_enc, grad_pred, grad_weight,
-                          grad_bias, workspace, options, Window{ranges, s_range});
+                          grad_bias, workspace, options, Window{ranges, s_range}, drop(dropout));
 }
 
 int rnnt_b200_joiner_last_launch_count(void) { return g_joiner_launches; }

@@ -6,8 +6,12 @@
 // by cp.async (zero-filled past the operand's extent) and read with ldmatrix (.trans for MN-major operands).
 // The pruned joiner (DESIGN.md §15) runs the same kernels with PRUNED = true over the rows (b, r, t), t fastest, of
 // the windows: row (b, r, t) is cell (t, ranges[b,t] + r), and px / py are written at the cell's dense index.
+// Dropout on h (DESIGN.md §16) is the DROP = true form of the two kernels that touch h element-wise, the h and ds
+// kernels: the keep bit of element (b, t, u, k) is a pure function of the seed and (dense cell index, k), so the
+// backward regenerates it and nothing is stored.
 #pragma once
 #include <cuda_bf16.h>
+#include <curand_philox4x32_x.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -39,6 +43,25 @@ struct Window {
     const int* ranges;   // [N, T]
     int R;
 };
+
+// Dropout on h: element k of the cell with dense index c is dropped iff word k & 3 of
+// Philox4x32-10(ctr = (k >> 2, c, 0, 0), key = (lo32(seed), hi32(seed))) is below thr; kept elements are scaled.
+// Calls without dropout pass {nullptr, 0, 1} and never read it.
+struct Drop {
+    const unsigned long long* seed;   // device pointer, read once per thread by the DROP kernels
+    uint32_t thr;                     // floor(p 2^32)
+    float scale;                      // 1 / (1 - p)
+};
+
+__device__ __forceinline__ uint2 drop_key(const Drop& d) {
+    const unsigned long long s = __ldg(d.seed);
+    return make_uint2((uint32_t)s, (uint32_t)(s >> 32));
+}
+
+// The four Philox words of columns 4 q .. 4 q + 3 of dense cell c.
+__device__ __forceinline__ uint4 drop_words(uint2 key, int q, int c) {
+    return curand_Philox4x32_10(make_uint4((uint32_t)q, (uint32_t)c, 0u, 0u), key);
+}
 
 struct Cell {
     int b, u, t;
@@ -233,12 +256,15 @@ __device__ __forceinline__ int load_rows(const Geo& g, const Window& w, int r0, 
 
 // h[r, :] = round_bf16(act(enc[b,t] + pred[b,u])) for a valid cell, 0 for padding and rows past the chunk; column H
 // is 1 (the dW contraction then yields dbias as its column H), columns H+1 .. Hp-1 are 0.  Padded rows of enc and
-// pred are never read.
-template <bool PRUNED>
+// pred are never read.  DROP: columns k < H of a valid cell hold h~ = keep ? round_bf16(h scale) : 0 (two Philox
+// calls per 8 columns); column H is never dropped.
+template <bool PRUNED, bool DROP = false>
 __global__ void __launch_bounds__(256) joiner_h_kernel(Geo g, int act, const bf16* __restrict__ enc,
                                                        const bf16* __restrict__ pred, bf16* __restrict__ h,
-                                                       int rows, Window w) {
+                                                       int rows, Window w, Drop d = Drop{nullptr, 0u, 1.f}) {
     const int groups = g.Hp / 8;
+    uint2 key = make_uint2(0u, 0u);
+    if constexpr (DROP) key = drop_key(d);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < (long long)rows * groups;
          i += (long long)gridDim.x * blockDim.x) {
     const int r = (int)(i / groups), k0 = (int)(i % groups) * 8;
@@ -257,6 +283,13 @@ __global__ void __launch_bounds__(256) joiner_h_kernel(Geo g, int act, const bf1
                 const float s = bf2f(ep[e]) + bf2f(pp[e]);
                 const float a = act == ACT_TANH ? tanhf(s) : ((s > 0.f || s != s) ? s : 0.f);
                 out[e] = __float2bfloat16_rn(a);
+            }
+            if constexpr (DROP) {
+                const uint4 x0 = drop_words(key, k0 >> 2, k.dense), x1 = drop_words(key, (k0 >> 2) + 1, k.dense);
+                const uint32_t x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+#pragma unroll
+                for (int e = 0; e < 8; ++e)
+                    out[e] = x[e] < d.thr ? __float2bfloat16_rn(0.f) : __float2bfloat16_rn(bf2f(out[e]) * d.scale);
             }
         }
     } else if (k0 == g.H) {
@@ -479,11 +512,16 @@ __global__ void __launch_bounds__(BM * 2) joiner_dlogits_kernel(Geo g, const bf1
 
 // ds[r, n] = (dlogits[r, :] W[:, n]) act'(h[r, n]) for a 64 x 64 tile (rows r, hidden units n); W is MN-major here.
 // Tiles whose rows are all padding write nothing: the reduction reads valid rows only.
-template <bool PRUNED>
+// DROP: ds[r, n] = (dlogits W)[r, n] m scale act'(s), with the keep bit m regenerated from the row's dense cell index
+// and n.  The scratch holds h~, not h: tanh recomputes h from the row's enc and pred elements exactly as the h kernel
+// forms it; relu takes m [s > 0] as [h~ > 0] (scale > 0, and a positive s rounds to a positive bf16 h).
+template <bool PRUNED, bool DROP = false>
 __global__ void __launch_bounds__(THREADS) joiner_ds_kernel(Geo g, int act, const bf16* __restrict__ dlog,
                                                             const bf16* __restrict__ W,
                                                             const bf16* __restrict__ h, float* __restrict__ ds,
-                                                            Window w) {
+                                                            Window w, Drop d = Drop{nullptr, 0u, 1.f},
+                                                            const bf16* __restrict__ enc = nullptr,
+                                                            const bf16* __restrict__ pred = nullptr) {
     extern __shared__ __align__(128) unsigned char smem_raw[];   // PAIR_STAGES A tiles, then as many B tiles
     bf16* sm = reinterpret_cast<bf16*>(smem_raw);
     __shared__ RowInfo<TILE, PRUNED> ri;
@@ -519,25 +557,63 @@ __global__ void __launch_bounds__(THREADS) joiner_ds_kernel(Geo g, int act, cons
         if ((it + 1) % STAGE_TILES == 0 || it + 1 == total) fold(tot, acc);
     }
     const int gq = lane >> 2, cq = lane & 3;
+    if constexpr (DROP) {
+        const uint2 key = drop_key(d);
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
+        for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int row = wm * 32 + mt * 16 + half * 8 + gq;
-            if (!(ri.flag[row] & 1)) continue;
-            const size_t r = (size_t)(r0 + row);
+            for (int half = 0; half < 2; ++half) {
+                const int row = wm * 32 + mt * 16 + half * 8 + gq;
+                if (!(ri.flag[row] & 1)) continue;
+                const size_t r = (size_t)(r0 + row);
+                const int c = ri.py(row), t = c % g.T, bu = c / g.T;   // the dense cell (b, u, t)
+                const bf16* er = enc + ((size_t)(bu / g.U) * g.T + t) * g.H;
+                const bf16* pr = pred + (size_t)bu * g.H;
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt) {
-                const int n = n0 + wn * 32 + nt * 8 + 2 * cq;
-                if (n >= g.H) continue;
-                const __nv_bfloat162 hv = *reinterpret_cast<const __nv_bfloat162*>(h + r * g.Hp + n);
-                const float h0 = __low2float(hv), h1 = __high2float(hv);
-                const float d0 = act == ACT_TANH ? 1.f - h0 * h0 : (h0 > 0.f ? 1.f : 0.f);
-                const float d1 = act == ACT_TANH ? 1.f - h1 * h1 : (h1 > 0.f ? 1.f : 0.f);
-                *reinterpret_cast<float2*>(ds + r * g.H + n) =
-                    make_float2(tot[mt][nt][half * 2] * d0, tot[mt][nt][half * 2 + 1] * d1);
+                for (int nt = 0; nt < 4; ++nt) {
+                    const int n = n0 + wn * 32 + nt * 8 + 2 * cq;
+                    if (n >= g.H) continue;
+                    const uint4 x = drop_words(key, n >> 2, c);   // n is even: words n & 3 and n & 3 + 1
+                    const float m0 = ((n & 2) ? x.z : x.x) < d.thr ? 0.f : d.scale;
+                    const float m1 = ((n & 2) ? x.w : x.y) < d.thr ? 0.f : d.scale;
+                    float d0, d1;
+                    if (act == ACT_TANH) {
+                        const __nv_bfloat162 ev = *reinterpret_cast<const __nv_bfloat162*>(er + n);
+                        const __nv_bfloat162 pv = *reinterpret_cast<const __nv_bfloat162*>(pr + n);
+                        const float h0 = bf2f(__float2bfloat16_rn(tanhf(__low2float(ev) + __low2float(pv))));
+                        const float h1 = bf2f(__float2bfloat16_rn(tanhf(__high2float(ev) + __high2float(pv))));
+                        d0 = (1.f - h0 * h0) * m0;
+                        d1 = (1.f - h1 * h1) * m1;
+                    } else {
+                        const __nv_bfloat162 hv = *reinterpret_cast<const __nv_bfloat162*>(h + r * g.Hp + n);
+                        d0 = __low2float(hv) > 0.f ? d.scale : 0.f;
+                        d1 = __high2float(hv) > 0.f ? d.scale : 0.f;
+                    }
+                    *reinterpret_cast<float2*>(ds + r * g.H + n) =
+                        make_float2(tot[mt][nt][half * 2] * d0, tot[mt][nt][half * 2 + 1] * d1);
+                }
             }
-        }
+    } else {
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                const int row = wm * 32 + mt * 16 + half * 8 + gq;
+                if (!(ri.flag[row] & 1)) continue;
+                const size_t r = (size_t)(r0 + row);
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt) {
+                    const int n = n0 + wn * 32 + nt * 8 + 2 * cq;
+                    if (n >= g.H) continue;
+                    const __nv_bfloat162 hv = *reinterpret_cast<const __nv_bfloat162*>(h + r * g.Hp + n);
+                    const float h0 = __low2float(hv), h1 = __high2float(hv);
+                    const float d0 = act == ACT_TANH ? 1.f - h0 * h0 : (h0 > 0.f ? 1.f : 0.f);
+                    const float d1 = act == ACT_TANH ? 1.f - h1 * h1 : (h1 > 0.f ? 1.f : 0.f);
+                    *reinterpret_cast<float2*>(ds + r * g.H + n) =
+                        make_float2(tot[mt][nt][half * 2] * d0, tot[mt][nt][half * 2 + 1] * d1);
+                }
+            }
+    }
 }
 
 // denc[b, t] += sum over the chunk's valid cells (b, u, t) of ds, in u order; dpred[b, u] += the same over t, in t

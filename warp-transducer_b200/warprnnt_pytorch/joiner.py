@@ -19,6 +19,11 @@ without the [N, T, R, V] logits of ``prune_joint_inputs`` -> joiner -> ``pruned_
 
     simple, ranges = add_joint_rnnt_loss_with_ranges(am_proj, lm_proj, labels, act_lens, label_lens, s_range=5)
     pruned = pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, 5)
+
+Both take NeMo's joint dropout, Sequential(act, Dropout(p), Linear), on the hidden activation (DESIGN.md §16), with
+the mask regenerated in the backward from a 64-bit seed instead of stored:
+
+    loss = joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, activation='relu', dropout=0.2)
 """
 import ctypes as C
 
@@ -51,6 +56,22 @@ _lib.rnnt_b200_pruned_joiner_backward.argtypes = [C.c_int, _P, _P, _P, _P, _P, _
                                                   C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                                   warp_rnnt.rnntOptions]
 
+
+class rnntJoinerDropout(C.Structure):
+    """include/rnnt.h struct rnntJoinerDropout, passed by value to the *_drop entries."""
+    _fields_ = [("p", C.c_float), ("seed", C.c_void_p)]
+
+
+def _drop_argtypes(plain):
+    """The *_drop entry's arguments: the plain entry's with the dropout struct before the workspace."""
+    return plain[:-2] + [rnntJoinerDropout] + plain[-2:]
+
+
+for _name in ("joiner_forward", "joiner_backward", "pruned_joiner_forward", "pruned_joiner_backward"):
+    _f = getattr(_lib, "rnnt_b200_%s_drop" % _name)
+    _f.restype = C.c_int
+    _f.argtypes = _drop_argtypes(getattr(_lib, "rnnt_b200_" + _name).argtypes)
+
 RNNT_B200_ACT_TANH, RNNT_B200_ACT_RELU = 0, 1
 _ACTIVATIONS = {'tanh': RNNT_B200_ACT_TANH, 'relu': RNNT_B200_ACT_RELU}
 
@@ -68,6 +89,37 @@ def _chunk(chunk_cells):
     if isinstance(chunk_cells, bool) or not isinstance(chunk_cells, int) or not 1 <= chunk_cells < 2 ** 31:
         raise ValueError("chunk_cells must be None or an int in [1, 2^31), got %r" % (chunk_cells,))
     return chunk_cells
+
+
+def dropout_p(dropout):
+    """The dropout probability as the C-ABI takes it (a float32 in [0, 1)); ValueError otherwise, a bool included."""
+    if isinstance(dropout, bool) or not isinstance(dropout, (int, float)):
+        raise ValueError("dropout must be a float in [0, 1), got %r" % (dropout,))
+    p = float(dropout)
+    if not (0.0 <= p < 1.0) or C.c_float(p).value >= 1.0:
+        raise ValueError("dropout must be a float in [0, 1), got %r" % (dropout,))
+    return p
+
+
+def _check_seed(seed):
+    """An explicit dropout seed: an int64 tensor of one element (the device is checked with the inputs')."""
+    if seed is None:
+        return
+    if not isinstance(seed, torch.Tensor) or seed.dtype is not torch.int64:
+        raise TypeError("dropout_seed must be None or an int64 tensor of one element, got %s"
+                        % (seed.dtype if isinstance(seed, torch.Tensor) else type(seed).__name__))
+    if seed.numel() != 1:
+        raise ValueError("dropout_seed must have one element, got shape %s" % (tuple(seed.shape),))
+
+
+def _seed_on(seed, device):
+    """The seed tensor a dropout call reads on the device: a fresh one from torch's CUDA generator when None (no host
+    synchronisation; torch.manual_seed reproduces it), else the caller's, which must be on the inputs' device."""
+    if seed is None:
+        return torch.empty(1, dtype=torch.int64, device=device).random_()
+    if not seed.is_cuda or seed.device != device:
+        raise RuntimeError("dropout_seed must be on the inputs' device %s, got %s" % (device, seed.device))
+    return seed.reshape(1).contiguous()
 
 
 def workspace_size(maxT, maxU, minibatch, hidden, alphabet_size, chunk_cells=None, s_range=None):
@@ -190,20 +242,31 @@ def _inputs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_ran
     return "rnnt_b200_pruned_joiner", head + [ranges.data_ptr(), s_range]
 
 
+def _drop(name, dropout, seed):
+    """The entry (plain, or its *_drop form when dropout > 0) and the trailing dropout argument, if any."""
+    if not dropout:
+        return getattr(_lib, name), []
+    if seed is None:
+        raise ValueError("a dropout call needs its seed tensor")
+    return getattr(_lib, name + "_drop"), [rnntJoinerDropout(dropout, seed.data_ptr())]
+
+
 def gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px, py, blank, activation,
-                       chunk_cells=None, workspace=None, ranges=None, s_range=None):
+                       chunk_cells=None, workspace=None, ranges=None, s_range=None, dropout=0.0, seed=None):
     """px [N, S, T] and py [N, S+1, T] (float32, every element written) from the joiner's inputs, checked by the
-    caller (include/rnnt.h rnnt_b200_joiner_forward; with ranges and s_range, rnnt_b200_pruned_joiner_forward).
-    Returns the workspace, which the backward reads."""
+    caller (include/rnnt.h rnnt_b200_joiner_forward; with ranges and s_range, rnnt_b200_pruned_joiner_forward; with
+    dropout > 0 their *_drop forms, reading the int64 seed tensor on the device).  Returns the workspace, which the
+    backward reads."""
     N, T, H = enc.shape
     U, V = pred.shape[1], weight.shape[0]
     name, head = _inputs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range)
+    fn, drop = _drop(name + "_forward", dropout, seed)
     with torch.cuda.device(enc.device):
         need = workspace_size(T, U, N, H, V, chunk_cells, s_range)
         if workspace is None or workspace.numel() < need:
             workspace = torch.empty(need, dtype=torch.uint8, device=enc.device)
-        st = getattr(_lib, name + "_forward")(activation_code(activation), *head, H, V, N, _chunk(chunk_cells),
-                                              _ptr(px), py.data_ptr(), workspace.data_ptr(), _options(enc, U, blank))
+        st = fn(activation_code(activation), *head, H, V, N, _chunk(chunk_cells), _ptr(px), py.data_ptr(), *drop,
+                workspace.data_ptr(), _options(enc, U, blank))
     if st != warp_rnnt.RNNT_STATUS_SUCCESS:
         raise RuntimeError(name + "_forward failed: " + warp_rnnt.status_string(st))
     return workspace
@@ -211,48 +274,53 @@ def gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px
 
 def gpu_joiner_backward(enc, pred, weight, bias, labels, act_lens, label_lens, dpx, dpy, grad_enc, grad_pred,
                         grad_weight, grad_bias, blank, activation, chunk_cells, workspace, ranges=None,
-                        s_range=None):
+                        s_range=None, dropout=0.0, seed=None):
     """The four bf16 gradients from dpx, dpy (float32, shaped as px, py) and the workspace of gpu_joiner_forward
-    with the same arguments (include/rnnt.h rnnt_b200_joiner_backward / rnnt_b200_pruned_joiner_backward)."""
+    with the same arguments, dropout and seed included (include/rnnt.h rnnt_b200_joiner_backward /
+    rnnt_b200_pruned_joiner_backward, or their *_drop forms)."""
     N, T, H = enc.shape
     U, V = pred.shape[1], weight.shape[0]
     name, head = _inputs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range)
+    fn, drop = _drop(name + "_backward", dropout, seed)
     with torch.cuda.device(enc.device):
-        st = getattr(_lib, name + "_backward")(activation_code(activation), *head, H, V, N, _chunk(chunk_cells),
-                                               _ptr(dpx), dpy.data_ptr(), grad_enc.data_ptr(), grad_pred.data_ptr(),
-                                               grad_weight.data_ptr(), _ptr(grad_bias), workspace.data_ptr(),
-                                               _options(enc, U, blank))
+        st = fn(activation_code(activation), *head, H, V, N, _chunk(chunk_cells), _ptr(dpx), dpy.data_ptr(),
+                grad_enc.data_ptr(), grad_pred.data_ptr(), grad_weight.data_ptr(), _ptr(grad_bias), *drop,
+                workspace.data_ptr(), _options(enc, U, blank))
     if st != warp_rnnt.RNNT_STATUS_SUCCESS:
         raise RuntimeError(name + "_backward failed: " + warp_rnnt.status_string(st))
 
 
 class _JoinerLogProbs(Function):
-    """The dense joiner (window None), or with a window (ranges, s_range) the pruned one.  forward: 2 launches per
-    chunk (the pruned call 1 more, the -inf fill), px / py and the per-row lse.  backward: 5 launches per chunk and 1
-    more, from the lse the forward left in the workspace."""
+    """The dense joiner (window None), or with a window (ranges, s_range) the pruned one; dropout > 0 on h with the
+    seed tensor (None: drawn from torch's CUDA generator).  forward: 2 launches per chunk (the pruned call 1 more,
+    the -inf fill), px / py and the per-row lse.  backward: 5 launches per chunk and 1 more, from the lse the forward
+    left in the workspace and the same seed."""
 
     @staticmethod
     def forward(ctx, enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, chunk_cells,
-                window=None):
+                window=None, dropout=0.0, seed=None):
+        dropout = dropout_p(dropout)
+        _check_seed(seed)
         length_check = _check_inputs(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
                                      chunk_cells, window)
+        seed = _seed_on(seed, enc.device) if dropout else None
         ranges, s_range = window if window is not None else (None, None)
         N, T, _ = enc.shape
         S = pred.shape[1] - 1
         px = torch.empty((N, S, T), dtype=torch.float32, device=enc.device)
         py = torch.empty((N, S + 1, T), dtype=torch.float32, device=enc.device)
         ws = gpu_joiner_forward(enc, pred, weight, bias, labels, act_lens, label_lens, px, py, blank, activation,
-                                chunk_cells, ranges=ranges, s_range=s_range)
+                                chunk_cells, ranges=ranges, s_range=s_range, dropout=dropout, seed=seed)
         length_check.finish()
-        ctx.save_for_backward(enc, pred, weight, bias, labels, act_lens, label_lens, ranges)
+        ctx.save_for_backward(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, seed)
         ctx.workspace = ws
-        ctx.args = (blank, activation, chunk_cells, s_range)
+        ctx.args = (blank, activation, chunk_cells, s_range, dropout)
         return px, py
 
     @staticmethod
     def backward(ctx, dpx, dpy):
-        enc, pred, weight, bias, labels, act_lens, label_lens, ranges = ctx.saved_tensors
-        blank, activation, chunk_cells, s_range = ctx.args
+        enc, pred, weight, bias, labels, act_lens, label_lens, ranges, seed = ctx.saved_tensors
+        blank, activation, chunk_cells, s_range, dropout = ctx.args
         N, T, _ = enc.shape
         S = pred.shape[1] - 1
         dpx = (torch.zeros((N, S, T), dtype=torch.float32, device=enc.device) if dpx is None
@@ -262,14 +330,16 @@ class _JoinerLogProbs(Function):
         grad_enc, grad_pred, grad_weight = torch.empty_like(enc), torch.empty_like(pred), torch.empty_like(weight)
         grad_bias = torch.empty_like(bias) if bias is not None else None
         gpu_joiner_backward(enc, pred, weight, bias, labels, act_lens, label_lens, dpx, dpy, grad_enc, grad_pred,
-                            grad_weight, grad_bias, blank, activation, chunk_cells, ctx.workspace, ranges, s_range)
+                            grad_weight, grad_bias, blank, activation, chunk_cells, ctx.workspace, ranges, s_range,
+                            dropout, seed)
         need = ctx.needs_input_grad
         return (grad_enc if need[0] else None, grad_pred if need[1] else None, grad_weight if need[2] else None,
-                grad_bias if bias is not None and need[3] else None, None, None, None, None, None, None, None)
+                grad_bias if bias is not None and need[3] else None, None, None, None, None, None, None, None, None,
+                None)
 
 
 def joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blank=0, *, activation='tanh',
-                     chunk_cells=None):
+                     chunk_cells=None, dropout=0.0, dropout_seed=None):
     """The lattice factors of the joiner  logits = weight act(enc[b,t] + pred[b,u]) + bias,  without the logits.
 
     enc [N, T, H], pred [N, U, H], weight [V, H], bias [V] or None: bf16, contiguous, on one CUDA device, with
@@ -284,13 +354,21 @@ def joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, blan
     backward returns bf16 gradients of enc, pred, weight and bias, accumulated in fp32 and bitwise deterministic for
     a given chunk_cells.
 
-    chunk_cells: cells per pass through the scratch; None keeps the scratch within 256 MiB."""
+    chunk_cells: cells per pass through the scratch; None keeps the scratch within 256 MiB.
+
+    dropout = p in [0, 1): NeMo's joint dropout on h (DESIGN.md §16).  The logits use h~ = keep ? round_bf16(h / (1 -
+    p)) : 0, the backward the same mask (regenerated, not stored) and act' from the undropped h.  Element k of cell
+    (b, t, u) is dropped iff word k & 3 of Philox4x32-10(ctr (k >> 2, (b U + u) T + t, 0, 0), key = the seed's two
+    halves) is below floor(p 2^32): the mask depends on the padded extents T and U, as eager dropout on [N, T, U, H]
+    does, and never on chunk_cells.  dropout_seed: None draws one int64 seed on the inputs' device from torch's CUDA
+    generator (no host sync; torch.manual_seed, CUDA-graph replays and torch.utils.checkpoint behave as for
+    nn.Dropout); or an int64 CUDA tensor of one element on that device.  dropout=0 is exactly the call without it."""
     return _JoinerLogProbs.apply(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
-                                 chunk_cells)
+                                 chunk_cells, None, dropout, dropout_seed)
 
 
 def pruned_joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range, blank=0, *,
-                            activation='tanh', chunk_cells=None):
+                            activation='tanh', chunk_cells=None, dropout=0.0, dropout_seed=None):
     """joiner_log_probs on the pruned lattice of pruned_rnnt_loss, without the [N, T, R, V] logits (DESIGN.md §15).
 
     ranges [N, T] int32 (contiguous, on the inputs' device) and s_range = R, a positive int: row (b, t, r), r < R,
@@ -299,9 +377,11 @@ def pruned_joiner_log_probs(enc, pred, weight, bias, labels, act_lens, label_len
     the cells a valid row covers, -inf everywhere else; dpx / dpy are read only on those cells.  The other arguments
     and the gradients are joiner_log_probs's; chunk_cells counts rows (b, t, r).  With s_range = U and ranges == 0
     both the factors and the gradients are bitwise joiner_log_probs's.  The alignment of the pruned lattice is
-    rnnt_lattice_forced_align(*pruned_joiner_log_probs(...), act_lens, label_lens)."""
+    rnnt_lattice_forced_align(*pruned_joiner_log_probs(...), act_lens, label_lens).  dropout and dropout_seed are
+    joiner_log_probs's; a row uses the mask of the cell it stands for, so with the same seed the result is the dense
+    one's on the covered cells."""
     return _JoinerLogProbs.apply(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation,
-                                 chunk_cells, (ranges, s_range))
+                                 chunk_cells, (ranges, s_range), dropout, dropout_seed)
 
 
 def _delay(px, act_lens, delay_penalty):
@@ -313,19 +393,21 @@ def _delay(px, act_lens, delay_penalty):
 
 
 def joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank=0, reduction='mean', *,
-                     activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+                     activation='tanh', rnnt_type='regular', delay_penalty=0.0, dropout=0.0, dropout_seed=None):
     """RNN-T loss of the joiner  logits = weight act(enc[b,t] + pred[b,u]) + bias  (see joiner_log_probs), without
     the [N, T, U, V] logits or their gradient:
 
         rnnt_lattice_loss(px + delay_penalty ((T_b - 1)/2 - t), py, act_lens, label_lens, reduction, rnnt_type)
 
-    on (px, py) = joiner_log_probs(...).  reduction, rnnt_type and delay_penalty are rnnt_loss's."""
+    on (px, py) = joiner_log_probs(...).  reduction, rnnt_type and delay_penalty are rnnt_loss's; dropout and
+    dropout_seed are joiner_log_probs's (applied whenever dropout > 0: the module form applies it in training only)."""
     return _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reduction, activation, rnnt_type,
-                 delay_penalty)
+                 delay_penalty, None, dropout, dropout_seed)
 
 
 def pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range, blank=0,
-                            reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+                            reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0,
+                            dropout=0.0, dropout_seed=None):
     """Pruned RNN-T loss of the joiner  logits = weight act(enc[b,t] + pred[b,u]) + bias  on the windows
     (ranges, s_range) of add_joint_rnnt_loss_with_ranges, without the [N, T, R, V] logits or their gradient: what
     prune_joint_inputs -> joiner -> pruned_rnnt_loss computes, as
@@ -333,19 +415,20 @@ def pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_len
         rnnt_lattice_loss(px + delay_penalty ((T_b - 1)/2 - t), py, act_lens, label_lens, reduction, rnnt_type)
 
     on (px, py) = pruned_joiner_log_probs(...).  An utterance whose windows leave no path costs +inf with zero
-    gradients.  reduction, rnnt_type and delay_penalty are pruned_rnnt_loss's."""
+    gradients.  reduction, rnnt_type and delay_penalty are pruned_rnnt_loss's; dropout and dropout_seed are
+    joiner_log_probs's."""
     return _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reduction, activation, rnnt_type,
-                 delay_penalty, (ranges, s_range))
+                 delay_penalty, (ranges, s_range), dropout, dropout_seed)
 
 
 def _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reduction, activation, rnnt_type,
-          delay_penalty, window=None):
+          delay_penalty, window=None, dropout=0.0, dropout_seed=None):
     warp_rnnt.rnnt_type_code(rnnt_type)
     warp_rnnt.lattice_options(delay_penalty)
     if reduction not in ('none', 'sum', 'mean'):
         raise ValueError("reduction must be 'none', 'sum' or 'mean'")
     px, py = _JoinerLogProbs.apply(enc, pred, weight, bias, labels, act_lens, label_lens, blank, activation, None,
-                                   window)
+                                   window, dropout, dropout_seed)
     if delay_penalty:
         px = _delay(px, act_lens, float(delay_penalty))
     return rnnt_lattice_loss(px, py, act_lens, label_lens, reduction, rnnt_type=rnnt_type)
@@ -353,9 +436,11 @@ def _loss(enc, pred, weight, bias, labels, act_lens, label_lens, blank, reductio
 
 class JoinerRNNTLoss(Module):
     """Module form of joiner_rnnt_loss: JoinerRNNTLoss(blank=0, reduction='mean', *, activation='tanh',
-    rnnt_type='regular', delay_penalty=0.0); forward(enc, pred, weight, bias, labels, act_lens, label_lens)."""
+    rnnt_type='regular', delay_penalty=0.0, dropout=0.0); forward(enc, pred, weight, bias, labels, act_lens,
+    label_lens).  dropout applies in training mode only, as nn.Dropout's, with a fresh seed per call."""
 
-    def __init__(self, blank=0, reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+    def __init__(self, blank=0, reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0,
+                 dropout=0.0):
         super().__init__()
         activation_code(activation)
         warp_rnnt.rnnt_type_code(rnnt_type)
@@ -364,19 +449,21 @@ class JoinerRNNTLoss(Module):
             raise ValueError("reduction must be 'none', 'sum' or 'mean'")
         self.blank, self.reduction = blank, reduction
         self.activation, self.rnnt_type, self.delay_penalty = activation, rnnt_type, delay_penalty
+        self.dropout = dropout_p(dropout)
 
     def forward(self, enc, pred, weight, bias, labels, act_lens, label_lens):
         return joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, self.blank, self.reduction,
                                 activation=self.activation, rnnt_type=self.rnnt_type,
-                                delay_penalty=self.delay_penalty)
+                                delay_penalty=self.delay_penalty, dropout=self.dropout if self.training else 0.0)
 
 
 class PrunedJoinerRNNTLoss(Module):
     """Module form of pruned_joiner_rnnt_loss: PrunedJoinerRNNTLoss(blank=0, reduction='mean', *, activation='tanh',
-    rnnt_type='regular', delay_penalty=0.0); forward(enc, pred, weight, bias, labels, act_lens, label_lens, ranges,
-    s_range)."""
+    rnnt_type='regular', delay_penalty=0.0, dropout=0.0); forward(enc, pred, weight, bias, labels, act_lens,
+    label_lens, ranges, s_range).  dropout applies in training mode only, as nn.Dropout's."""
 
-    def __init__(self, blank=0, reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0):
+    def __init__(self, blank=0, reduction='mean', *, activation='tanh', rnnt_type='regular', delay_penalty=0.0,
+                 dropout=0.0):
         super().__init__()
         activation_code(activation)
         warp_rnnt.rnnt_type_code(rnnt_type)
@@ -385,8 +472,10 @@ class PrunedJoinerRNNTLoss(Module):
             raise ValueError("reduction must be 'none', 'sum' or 'mean'")
         self.blank, self.reduction = blank, reduction
         self.activation, self.rnnt_type, self.delay_penalty = activation, rnnt_type, delay_penalty
+        self.dropout = dropout_p(dropout)
 
     def forward(self, enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range):
         return pruned_joiner_rnnt_loss(enc, pred, weight, bias, labels, act_lens, label_lens, ranges, s_range,
                                        self.blank, self.reduction, activation=self.activation,
-                                       rnnt_type=self.rnnt_type, delay_penalty=self.delay_penalty)
+                                       rnnt_type=self.rnnt_type, delay_penalty=self.delay_penalty,
+                                       dropout=self.dropout if self.training else 0.0)
