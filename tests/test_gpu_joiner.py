@@ -15,6 +15,7 @@ import torch
 import torch.nn.functional as F
 
 import align_reference as ar
+import joiner_blocks as jb
 import joiner_reference as jr
 import lattice_reference as lr
 
@@ -77,14 +78,14 @@ def check_factors(px, py, px_ref, py_ref, bar):
         assert (err <= b[ok]).all(), (err.max().item(), (err / b[ok]).max().item())
 
 
-def check_gradients(got, h, weight, bias, dl, dl_err, activation, chunks, slabs=16):
-    """Each of (d_enc, d_pred, d_weight, d_bias) within its bar of the fp64 contraction of dl."""
-    N, T, U, _ = h.shape
+def gradient_bars(ht, ag, weight, dl, dl_err, chunks, slabs=16):
+    """fp64 (d_enc, d_pred, d_weight, d_bias) of dl with ht as dW's operand and ag as ds's factor, and each one's bar
+    without the final bf16 rounding 2^-8 |ref|."""
+    N, T, U, _ = ht.shape
     V = weight.shape[0]
-    ha, wa, dla = h.double().abs(), weight.double().abs(), dl.abs()
-    ag = jr.act_grad(h, activation)
+    ha, wa, dla = ht.double().abs(), weight.double().abs(), dl.abs()
     ds_ref = (dl @ weight.double()) * ag
-    ref = (ds_ref.sum(2), ds_ref.sum(1), torch.einsum('ntuv,ntuh->vh', dl, h.double()), dl.sum((0, 1, 2)))
+    ref = (ds_ref.sum(2), ds_ref.sum(1), torch.einsum('ntuv,ntuh->vh', dl, ht.double()), dl.sum((0, 1, 2)))
     g_dw = (32 + N * T * U / 256 + slabs + chunks) * 2 * U_
     g_ds = (32 + V / 256) * 2 * U_
     b_ds = ((dl_err @ wa) + g_ds * (dla @ wa)) * ag
@@ -92,6 +93,12 @@ def check_gradients(got, h, weight, bias, dl, dl_err, activation, chunks, slabs=
             b_ds.sum(1) + (T + chunks) * 2 * U_ * ds_ref.abs().sum(1),
             torch.einsum('ntuv,ntuh->vh', dl_err, ha) + g_dw * torch.einsum('ntuv,ntuh->vh', dla, ha),
             dl_err.sum((0, 1, 2)) + g_dw * dla.sum((0, 1, 2)))
+    return ref, bars
+
+
+def check_gradients(got, h, weight, bias, dl, dl_err, activation, chunks, slabs=16):
+    """Each of (d_enc, d_pred, d_weight, d_bias) within its bar of the fp64 contraction of dl."""
+    ref, bars = gradient_bars(h, jr.act_grad(h, activation), weight, dl, dl_err, chunks, slabs)
     for name, g, r, b in zip(("d_enc", "d_pred", "d_weight", "d_bias"), got, ref, bars):
         if g is None:
             continue
@@ -205,18 +212,9 @@ def test_label_outside_the_alphabet():
 
 
 def _plan_h_offset(N, T, U, H, V, chunk):
-    """Byte offset of the h scratch in the workspace (rnnt_joiner.cu, plan())."""
-    up = lambda x, a: -(-x // a) * a
-    Hp, Vp = up(H + 1, 64), up(V, 64)
-    cells = N * T * U
-    chunk = min(chunk, cells)
-    rows = up(chunk, 128)
-    slabs = min(-(-264 // ((Vp // 64) * (Hp // 64))), 16, rows // 64)
-    o = up(cells * 4, 256)
-    o = up(o + N * T * H * 4, 256)
-    o = up(o + N * U * H * 4, 256)
-    o = up(o + slabs * Vp * Hp * 4, 256)
-    return o, Hp
+    """Byte offset of the h scratch in the workspace (rnnt_joiner.cu, plan(); mirrored in joiner_blocks.plan)."""
+    p = jb.plan(T, U, N, H, V, chunk)
+    return p.h, p.Hp
 
 
 @pytest.mark.parametrize("activation", ["tanh", "relu"])

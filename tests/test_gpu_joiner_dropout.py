@@ -11,6 +11,7 @@ import torch
 import torch.nn.functional as F
 
 import dropout_reference as dr
+import joiner_blocks as jb
 import joiner_reference as jr
 import lattice_reference as lr
 import pruned_joiner_reference as pjr
@@ -110,16 +111,10 @@ def full_check(inputs, blank, activation, p, seed, chunk_cells=None, window=None
 # 1. the kernel's h~ is the reference's bit for bit
 
 def _h_offset(N, T, U, rows_per_frame, H, V, chunk):
-    """Byte offset of the h scratch in the workspace (rnnt_joiner.cu, plan()), and Hp."""
-    up = lambda x, a: -(-x // a) * a
-    Hp, Vp = up(H + 1, 64), up(V, 64)
-    cells = N * T * rows_per_frame
-    rows = up(min(chunk, cells), 128)
-    slabs = min(-(-264 // ((Vp // 64) * (Hp // 64))), 16, rows // 64)
-    o = 0
-    for n in (cells * 4, N * T * H * 4, N * U * H * 4, slabs * Vp * Hp * 4):
-        o = up(o + n, 256)
-    return o, Hp
+    """Byte offset of the h scratch in the workspace (rnnt_joiner.cu, plan(); mirrored in joiner_blocks.plan), and
+    Hp."""
+    p = jb.plan(T, U, N, H, V, chunk, rows_per_frame)
+    return p.h, p.Hp
 
 
 @pytest.mark.parametrize("pruned", [False, True])
